@@ -7,8 +7,9 @@ per-Gaussian gradients into one flat buffer and the ranks all-reduce it over NCC
 Workload at N=1: BASELINE.json configs[1] — 100k Gaussians, 800x800, SH degree 3 (synthetic DreamGaussian-like cloud,
 dreamgaussian_b200/scene.py).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            # our sm_100a path (the product)
+  python bench.py [--gpus N] [--steps K] [--warmup W]            # our sm_90a path (the product)
   python bench.py --impl reference ...                           # the CPU oracle port, timed on the host cores
+  python bench.py ... --dump-outputs DIR                         # also write the last timed step's gradients as DIR/*.npy
 
 One JSON line on stdout (rank 0).  See DESIGN.md "Measurement" for every field.
 """
@@ -55,6 +56,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-rows", action="store_true", help="skip the short measurements of the SURVEY §8f rows (f1-f4)")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (the per-Gaussian gradients) as DIR/<name>.npy")
     a = ap.parse_args()
     w = WORKLOADS[a.workload]
     for k in ("points", "res", "views_per_gpu", "views", "steps"):
@@ -90,8 +93,26 @@ def kernel_algorithmic_bytes(name, P, M, H, W, n_inst):
     return table.get(name)
 
 
+def dump_outputs(out_dir, grads, cap_bytes=64 << 20):
+    """What a caller of the timed path receives from one step: the per-Gaussian gradients of the flat buffer, one float32 file
+    per op input.  Above cap_bytes in all, the same fixed, seeded sample of Gaussians is taken from every array and its row
+    indices are written too (sample_rows.npy, float64)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v for k, v in grads.views.items() if v is not None}
+    row_bytes = sum(v[0].numel() for v in arrays.values()) * 4 if grads.P else 0
+    rows = None
+    if row_bytes * grads.P > cap_bytes:
+        n = int(cap_bytes * 0.9) // (row_bytes + 8)
+        pick = np.sort(np.random.default_rng(0).choice(grads.P, size=n, replace=False))
+        np.save(os.path.join(out_dir, "sample_rows.npy"), pick.astype(np.float64))
+        rows = torch.from_numpy(pick).to(grads.flat.device)
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, "grad_%s.npy" % k), (v if rows is None else v.index_select(0, rows)).float().cpu().numpy())
+
+
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -474,7 +495,7 @@ def run_ours(a, rank, world, local_rank):
         campos=t(c.camera_center), prefiltered=False, debug=False) for c in cams]
     ups_d = [(t(u[0]), None, t(u[2])) for u in ups]
     vsr = multiview.ViewShardedRasterizer(P, M, dev)
-    flush_buf = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)    # > 126 MB L2
+    flush_buf = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)    # several times the 50 MB L2 of an H100
 
     def local_views(i):
         return [((i * world + rank) * vpg + k) % len(settings) for k in range(vpg)]
@@ -527,6 +548,8 @@ def run_ours(a, rank, world, local_rank):
     ms_total = float(ms_t.item())
     ms_per_step = ms_total / a.steps
     value = P * vpg * world * a.steps / (ms_total * 1e-3)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, vsr.grads)          # before the passes below overwrite the buffer
 
     # ---------------- per-kernel CUDA-event timing (separate pass, same workload, this rank's stream) ----------------
     kern = {}
@@ -723,8 +746,8 @@ def run_ours(a, rank, world, local_rank):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (of fallback)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet: 3350 GB/s HBM3"
     known = {k: v for k, v in kern.items() if kernel_algorithmic_bytes(k, P, M, H, W, n_inst)}
     dom = max(known, key=known.get) if known else None
     roof = {"bound": "hbm", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None, "traffic": None, "peak_source": peak_src}

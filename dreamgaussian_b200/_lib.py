@@ -1,7 +1,7 @@
 """ctypes binding of libdgr_b200.so (the C ABI declared in include/dgr_b200.h).
 
 There is NO fallback: if the shared library is missing or does not load, importing the compute entry points raises.
-The library is built in-tree by ``dreamgaussian_b200.build`` (nvcc, sm_100a).
+The library is built in-tree by ``dreamgaussian_b200.build`` (nvcc, sm_90a).
 """
 import ctypes
 import os

@@ -1,4 +1,4 @@
-"""Build recipe of libdgr_b200.so: one nvcc invocation, sm_100a only, in-tree output (dreamgaussian_b200/lib/).
+"""Build recipe of libdgr_b200.so: one nvcc invocation, sm_90a only, in-tree output (dreamgaussian_b200/lib/).
 
 No torch headers are involved: the library is a plain C-ABI CUDA shared object (include/dgr_b200.h).
 nvcc cross-compiles on a machine without a GPU, so this runs in CI and in __graft_entry__.build().
@@ -14,7 +14,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdgr_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr", "-Xptxas", "-v", "-ldl",
 ]

@@ -262,9 +262,9 @@ using SmB = SortSmem<kSortBigThreads, kSortBigCap, kSortBigBuckets>;
 // grids are properties of a (function, device) pair, so they are kept per device ordinal and set up once under a mutex.
 struct DevInfo {
     bool ready = false;
-    int sms = 148;
-    size_t l2_bytes = 126u << 20;
-    int big_grid = 148;               // big-tile sorter: one CTA per SM
+    int sms = 132;                    // H100 SXM until the device is queried
+    size_t l2_bytes = 50u << 20;
+    int big_grid = 132;               // big-tile sorter: one CTA per SM
     std::map<const void *, int> grids;   // persistent (occupancy x SMs) grid of every render kernel instantiation used so far
 };
 constexpr int kMaxDevices = 64;
@@ -443,8 +443,8 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v
     }
     // Record staging of the render kernels.  A sorted copy of the records (written by the sort kernel, read with one contiguous
     // bulk-TMA copy per 32 records) is the fast path while that copy lives in L2; once it is several times the L2 size the
-    // sort kernel's gather + write becomes the long pole (2M / 1600^2: 457 vs 164 us) and staging by id wins although a
-    // chunk then takes 32 small bulk copies (B200: 78 vs 21 ns per chunk per SM, profiles/r2_tma_gather_probe.txt).
+    // sort kernel's gather + write becomes the long pole and staging by id wins although a chunk then takes 32 small bulk
+    // copies (tools/tma_gather_probe.cu times both).  The threshold follows the device's L2 size (50 MB on an H100).
     const int lz = g_lazy.load();
     const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
     if (g->P > 0 && capacity > 0) {
@@ -613,7 +613,7 @@ int dgr_dist_cuda2(int32_t P, const float *points, float *mean_dists, void *scra
     DGR_CUDA(cudaMemsetAsync(cell_start, 0, (L.cap + 1) * 4, st));
     DGR_CUDA(cudaMemsetAsync(cell_fill, 0, L.cap * 4, st));
     const int nb = (P + 255) / 256;
-    const int nb_bbox = nb < 4 * (dev_info() ? dev_info()->sms : 148) ? nb : 4 * (dev_info() ? dev_info()->sms : 148);
+    const int nb_bbox = nb < 4 * (dev_info() ? dev_info()->sms : 132) ? nb : 4 * (dev_info() ? dev_info()->sms : 132);
     const size_t n_scan = L.cap + 1;
     DGR_KERNEL("knn_bbox", st, 0, knn_bbox_kernel<<<nb_bbox, 256, 0, st>>>(P, points, grid));
     DGR_KERNEL("knn_grid", st, 0, knn_grid_kernel<<<1, 1, 0, st>>>(P, (unsigned)L.cap, grid));
@@ -653,7 +653,7 @@ int dgr_extract_fields(int32_t P, const float *xyz, const float *opacity_raw, co
     DGR_CUDA(cudaMemsetAsync(cell_fill, 0, L.cells * 4, st));
     const int nbk = P > 0 ? (P + 255) / 256 : 1;
     if (P > 0) {
-        const int nb_bbox = nbk < 4 * (dev_info() ? dev_info()->sms : 148) ? nbk : 4 * (dev_info() ? dev_info()->sms : 148);
+        const int nb_bbox = nbk < 4 * (dev_info() ? dev_info()->sms : 132) ? nbk : 4 * (dev_info() ? dev_info()->sms : 132);
         DGR_KERNEL("fields_bbox", st, 0, fields_bbox_kernel<<<nb_bbox, 256, 0, st>>>(P, xyz, opacity_raw, hdr));
     }
     DGR_KERNEL("fields_prep", st, 0, fields_prep_kernel<<<nbk, 256, 0, st>>>(P, xyz, opacity_raw, scaling_raw, rotation_raw, hdr, num_blocks,
@@ -692,7 +692,7 @@ int dgr_adam_step(const DgrAdamGroup *groups, int32_t n_groups, double beta1, do
     if (run == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     unsigned long long blocks = (run + 255) / 256;
-    const unsigned long long cap = (unsigned long long)(dev_info() ? dev_info()->sms : 148) * 16;
+    const unsigned long long cap = (unsigned long long)(dev_info() ? dev_info()->sms : 132) * 16;
     if (blocks > cap) blocks = cap;
     DGR_KERNEL("adam_multi", st, 0, adam_multi_kernel<<<(unsigned)blocks, 256, 0, st>>>(G, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps));
     return 0;

@@ -441,15 +441,20 @@ tile_sort_gather_kernel(const TileWork *__restrict__ work, const uint2 *__restri
     pdl_trigger();
     pdl_wait();
     const unsigned n_tiles = __ldcg(&work->n_nonempty);
+    // the look-ahead range travels through shared memory: held in registers across the sort it spills on sm_90 (32-register cap)
+    __shared__ uint2 s_range[2];
     unsigned i = blockIdx.x;
-    uint2 r = i < n_tiles ? __ldcg(order_ranges + i) : make_uint2(0u, 0u);
-    while (i < n_tiles) {
+    if (threadIdx.x == 0) s_range[0] = i < n_tiles ? __ldcg(order_ranges + i) : make_uint2(0u, 0u);
+    __syncthreads();
+    for (int b = 0; i < n_tiles; b ^= 1) {
         const unsigned inext = i + gridDim.x;
-        const uint2 rnext = inext < n_tiles ? __ldcg(order_ranges + inext) : make_uint2(0u, 0u);
+        if (threadIdx.x == 0) s_range[b ^ 1] = inext < n_tiles ? __ldcg(order_ranges + inext) : make_uint2(0u, 0u);
+        const uint2 r = s_range[b];
         const int n = (int)(r.y - r.x);
         if (n > 0 && n <= kSortSmallCap)
             sort_gather_tile<kSortSmallThreads, kSortSmallCap, NBK>(r, keys, rec, ids_sorted, rec_sorted, s_sort, gather != 0);
-        i = inext; r = rnext;
+        __syncthreads();                               // every thread has read s_range[b] before thread 0 refills it
+        i = inext;
     }
 }
 

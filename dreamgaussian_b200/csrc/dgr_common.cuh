@@ -1,4 +1,4 @@
-// dgr_common.cuh — shared definitions of the sm_100a rasterizer kernels: scratch layouts, PTX wrappers
+// dgr_common.cuh — shared definitions of the sm_90a rasterizer kernels: scratch layouts, PTX wrappers
 // (mbarrier + 1-D bulk TMA), small math helpers.
 #pragma once
 #include <cuda_runtime.h>
@@ -218,7 +218,7 @@ __device__ __forceinline__ bool ellipse_hits_rect(float cx, float cy, float nA, 
 // The tiles a Gaussian is binned into: those of its opacity-aware pixel AABB (which already carries the reference's
 // 3-sigma tile-rect clip).  Used — with the SAME packed record values — by the preprocess histogram and by the emit kernel,
 // so both make identical decisions.  (The exact ellipse test is applied later, per warp sub-tile, in the render kernels:
-// measured on B200 it costs more in these two latency-bound per-Gaussian loops than the ~8% of instances it removes.)
+// it costs more in these two latency-bound per-Gaussian loops than the ~8% of instances it removes.)
 template <class F>
 __device__ __forceinline__ void for_each_touched_tile(unsigned ax, unsigned ay, int gx, F f) {
     const int bx0 = (int)(ax & 0xffffu), bx1 = (int)(ax >> 16), by0 = (int)(ay & 0xffffu), by1 = (int)(ay >> 16);

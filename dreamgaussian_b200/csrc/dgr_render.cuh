@@ -1,8 +1,8 @@
 // dgr_render.cuh — per-tile front-to-back compositing (A4) and its reverse-traversal backward (A5).
 //
-// B200 design (not the reference's one-thread-per-pixel CTA with a cooperative fetch and a block barrier per batch):
+// Design (not the reference's one-thread-per-pixel CTA with a cooperative fetch and a block barrier per batch):
 //   * the unit of work is ONE WARP x ONE SUB-TILE (32*PPL pixels of a 16x16 tile).  A persistent grid (as many CTAs as
-//     fit on the 148 SMs) of independent warps pulls (tile, sub-tile) items, heaviest tile first, from an atomic counter in
+//     fit on the SMs) of independent warps pulls (tile, sub-tile) items, heaviest tile first, from an atomic counter in
 //     global memory: no CTA-level coupling, no block barrier, no idle warps waiting for a slower sibling, and the SMs stay
 //     evenly loaded although tile populations differ by orders of magnitude;
 //   * a tile's depth-sorted 48-byte records are one contiguous block.  Each warp streams it through its OWN shared-memory

@@ -26,7 +26,7 @@ const float *fptr(const OptTensor &t) { return (t.has_value() && t->defined() &&
 float *fptr_mut(const OptTensor &t) { return (t.has_value() && t->defined() && t->numel() > 0) ? t->data_ptr<float>() : nullptr; }
 
 Tensor dev_f32(const Tensor &t, const char *name) {
-    TORCH_CHECK(t.is_cuda(), name, " is on ", t.device(), ": this rasterizer has no CPU path (it runs as sm_100a CUDA kernels in libdgr_b200.so)");
+    TORCH_CHECK(t.is_cuda(), name, " is on ", t.device(), ": this rasterizer has no CPU path (it runs as sm_90a CUDA kernels in libdgr_b200.so)");
     Tensor r = t.scalar_type() == torch::kFloat32 ? t : t.to(torch::kFloat32);
     r = r.contiguous();
     // the kernels read rotations / SH rows with 128-bit loads and stage inputs with bulk TMA: a view that starts off a 16-byte

@@ -8,7 +8,7 @@ Drop-in for the import at /root/reference/gs_renderer.py:10-13 and the call at g
 
 Same names, argument meaning, return shapes/dtypes (color [3,H,W], radii int32 [P], depth [1,H,W], alpha [1,H,W]) and
 error behaviour (the two "Please provide ..." exceptions) as the un-vendored package the reference imports [EXT].
-All arithmetic runs in libdgr_b200.so (hand-written sm_100a CUDA) through the C ABI of include/dgr_b200.h; torch is
+All arithmetic runs in libdgr_b200.so (hand-written sm_90a CUDA) through the C ABI of include/dgr_b200.h; torch is
 used for device memory, the current stream and autograd plumbing only.  There is no CPU path: non-CUDA tensors raise.
 """
 import ctypes
@@ -95,7 +95,7 @@ def _dev_f32(t: torch.Tensor, name: str) -> torch.Tensor:
         raise TypeError("%s must be a torch.Tensor" % name)
     if not t.is_cuda:
         raise RuntimeError(
-            "%s is on %s: this rasterizer has no CPU path (it runs as sm_100a CUDA kernels in libdgr_b200.so)" % (name, t.device))
+            "%s is on %s: this rasterizer has no CPU path (it runs as sm_90a CUDA kernels in libdgr_b200.so)" % (name, t.device))
     if t.dtype != torch.float32:
         t = t.float()
     return _aligned16(t.contiguous())

@@ -32,7 +32,7 @@ MAX_AMBIG_FRAC = 0.04
 TIE_SLACK_FACTOR = 1.5
 # float32 CUDA vs the float32 build of the oracle (compare_f32): NO decision-ambiguity exemption, only float32 depth-key
 # ties (two consecutive contributors of a pixel whose view depths differ by < 1e-6 relative: either order is a valid
-# float32 result) are set aside.  Bounds from tools/parity_report.py on B200 (profiles/r2_parity_report.json).
+# float32 result) are set aside.  Bounds from tools/parity_report.py.
 F32_IMG_ATOL = 2e-4            # every non-tie pixel ...
 F32_IMG_OUTLIERS = 2e-5        # ... except this fraction of them (alpha >= 1/255 / T-stop decisions taken the other way) ...
 F32_IMG_OUTLIER_ATOL = 1e-2    # ... which stay below this

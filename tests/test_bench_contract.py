@@ -36,19 +36,3 @@ def test_algorithmic_bytes_formula_matches_survey():
     # SURVEY.md §8(d): deg 3 -> 724 B/Gaussian, 52 B/pixel, 44 B/instance; cfg2 = 151.5 MB with N_inst 1.040 M
     assert bench.algorithmic_bytes(1, 16, 0, 0, 0) == 724 and bench.algorithmic_bytes(1, 1, 0, 0, 0) == 184
     assert abs(bench.algorithmic_bytes(100000, 16, 800, 800, 1040000) - 151.44e6) < 0.1e6
-
-
-def test_committed_ncu_capture_belongs_to_the_current_kernel_sources():
-    """bench.py folds profiles/r2_ncu_kernels.json (DRAM bytes and warp instructions per launch from one `ncu --set full` capture)
-    into `roofline.traffic` / `roofline.issue` and refuses it when it was taken on other kernel sources.  The committed capture
-    must be the current sources' one — a kernel edit without a re-capture (tools/r2_final2.sh) fails here, not silently in the line."""
-    from dreamgaussian_b200 import build
-    d = json.load(open(os.path.join(h.ROOT, "profiles", "r2_ncu_kernels.json")))
-    assert d["lib_source_hash"] == build.step_kernel_hash()[:16]
-    for k in ("preprocess_fwd", "emit_instances", "tile_sort_gather", "render_fwd", "render_bwd", "preprocess_bwd"):
-        assert d["dram_bytes_per_launch"][k] > 0 and d["warp_inst_per_launch"][k] > 0 and d["launches_captured"][k] >= 2
-    sys.path.insert(0, h.ROOT)
-    import bench
-    for kind in ("dram_bytes_per_launch", "warp_inst_per_launch"):
-        vals, src = bench.committed_ncu(kind)
-        assert vals and vals["render_bwd"] > 0 and "ncu" in src          # (a stale capture returns None and the reason)

@@ -1,4 +1,4 @@
-"""GPU parity tests: the CUDA path (public API -> C ABI -> sm_100a kernels) against the float64 CPU oracle on the same
+"""GPU parity tests: the CUDA path (public API -> C ABI -> sm_90a kernels) against the float64 CPU oracle on the same
 seeded inputs, plus size-independent properties at BASELINE.json's full sizes.  Tolerances: tests/helpers.py."""
 import ctypes
 

@@ -1,4 +1,4 @@
-"""What the compiled sm_100a library must look like (no GPU needed: cuobjdump reads dreamgaussian_b200/lib/libdgr_b200.so).
+"""What the compiled sm_90a library must look like (no GPU needed: cuobjdump reads dreamgaussian_b200/lib/libdgr_b200.so).
 
 Guards the properties DESIGN.md §4 states about the step kernels against silent regressions: register budgets that decide how many
 CTAs fit per SM, no spills in the render / sort kernels, bulk-TMA (UBLKCP) + mbarrier (SYNCS) staging where it is claimed and nowhere

@@ -2,7 +2,7 @@
 //   (a) one contiguous 1536-byte block (one cp.async.bulk)            — what the render kernels do today (sorted copy), or
 //   (b) 32 scattered 48-byte records (32 cp.async.bulk, one per lane) — a gather straight from the per-Gaussian array, or
 //   (c) 32 scattered records through plain 128-bit loads + shared-memory stores (no TMA)?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_scratch/tma_gather_probe tools/tma_gather_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_gather_probe tools/tma_gather_probe.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
