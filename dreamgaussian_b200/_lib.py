@@ -9,7 +9,7 @@ import os
 from . import build as _build
 
 c_f32p = ctypes.c_void_p  # device pointers travel as integers
-ABI_VERSION = 4          # include/dgr_b200.h DGR_ABI_VERSION
+ABI_VERSION = 5          # include/dgr_b200.h DGR_ABI_VERSION
 
 
 class DgrSettings(ctypes.Structure):
@@ -123,7 +123,7 @@ def load():
     lib.dgr_forward_render.argtypes = [ctypes.POINTER(DgrSettings), ctypes.POINTER(DgrGaussians), vp, vp, u64, vp,
                                        ctypes.POINTER(DgrImages), i32, vp, u64, vp, vp]
     lib.dgr_backward.restype = ctypes.c_int
-    lib.dgr_backward.argtypes = [ctypes.POINTER(DgrSettings), ctypes.POINTER(DgrGaussians), vp, vp, u64, vp, vp, vp,
+    lib.dgr_backward.argtypes = [ctypes.POINTER(DgrSettings), ctypes.POINTER(DgrGaussians), vp, vp, u64, i32, vp, vp, vp,
                                  ctypes.POINTER(DgrImageGrads), ctypes.POINTER(DgrGaussianGrads), vp]
     lib.dgr_knn_scratch_bytes.restype = ctypes.c_size_t
     lib.dgr_knn_scratch_bytes.argtypes = [i32]

@@ -248,10 +248,9 @@ __global__ void debug_geom_kernel(int P, const Rec *rec, const unsigned *touched
 // tuning knobs (dgr_set_tuning): pixels per lane of the render kernels, heaviest-first tile order on/off.  Atomics: any host
 // thread may change them while another launches (each launch reads every knob once).
 std::atomic<int> g_ppl_fwd{1}, g_ppl_bwd{1}, g_u_fwd{0}, g_u_bwd{0};      // u = 0: the default batching of that sub-tile shape
-std::atomic<bool> g_no_order{false};
-std::atomic<int> g_two_ended{0};
-std::atomic<int> g_cost_order{1};
-std::atomic<int> g_lazy{0};            // record staging of the render kernels: 0 = by id when the sorted copy would exceed 2x L2, 1 = always sorted copy, 2 = always by id      // backward work ordered by the cost the forward measured (dgr_render.cuh)       // work queue of the render kernels consumed from both ends (dgr_render.cuh)
+std::atomic<int> g_two_ended{0};       // work queue of the render kernels consumed from both ends (dgr_render.cuh)
+std::atomic<int> g_cost_order{1};      // backward work ordered by the cost the forward measured (dgr_render.cuh)
+std::atomic<int> g_lazy{0};            // record staging of the render kernels: 0 = by id when the sorted copy would exceed 2x L2, 1 = always sorted copy, 2 = always by id
 std::atomic<int> g_cta_fwd{0}, g_cta_bwd{0};   // persistent CTAs per SM of the render kernels (0 = as many as fit)
 
 using SmS = SortSmem<kSortSmallThreads, kSortSmallCap, kSortSmallBuckets>;
@@ -339,7 +338,6 @@ int dgr_profile_collect(char *names, size_t names_bytes, float *ms, int max) {
 int dgr_set_tuning(int ppl_fwd, int ppl_bwd, int tile_order) {
     if ((ppl_fwd != 1 && ppl_fwd != 2 && ppl_fwd != 4) || (ppl_bwd != 1 && ppl_bwd != 2 && ppl_bwd != 4)) return fail(-1, "ppl must be 1, 2 or 4");
     g_ppl_fwd = ppl_fwd; g_ppl_bwd = ppl_bwd == 4 ? 2 : ppl_bwd;          // the backward has 8x4 and 8x8 sub-tiles
-    g_no_order = (tile_order & 3) == 0;
     g_pdl = (tile_order & 8) ? 0 : 1;                   // bit 3: programmatic dependent launches OFF (A/B switch)
     g_u_fwd = (tile_order >> 4) & 7;                    // bits 4-6 / 8-10: hits evaluated together by the forward / backward
     g_u_bwd = (tile_order >> 8) & 7;                    // render kernels (1, 2 or 4; 0 = default of the sub-tile shape)
@@ -445,8 +443,11 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v
     // bulk-TMA copy per 32 records) is the fast path while that copy lives in L2; once it is several times the L2 size the
     // sort kernel's gather + write becomes the long pole and staging by id wins although a chunk then takes 32 small bulk
     // copies (tools/tma_gather_probe.cu times both).  The threshold follows the device's L2 size (50 MB on an H100).
+    // Decided here once: the backward of this call must stage its records the same way (the sorted copy is not written when
+    // staging by id), whatever the knobs say by then — the caller hands counts_host[3] to dgr_backward.
     const int lz = g_lazy.load();
     const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
+    if (counts_host) counts_host[3] = lazy ? DGR_STAGING_BY_ID : DGR_STAGING_SORTED;
     if (g->P > 0 && capacity > 0) {
         if (g_sort_fine.load()) {
             const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBucketsFine>, kSortSmallThreads, SmSF::bytes));
@@ -513,13 +514,15 @@ static int flat_segs(int32_t n_seg, const int64_t *seg_off, const int32_t *seg_s
 }
 
 int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
-                 const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                 int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
                  const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_backward");
     (void)out_alpha;
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
+    if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
+        return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
     if (g->P == 0) return 0;
     if (!radii) return fail(-1, "radii is NULL");
     if (int e = check_push(gout->push, g->P)) return e;
@@ -563,9 +566,8 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
                             reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, grad_rec)); \
     } while (0)
 #define DGR_RENDER_BWD(PPL_, U_) do { if (lazy) DGR_RENDER_BWD_L(PPL_, U_, true); else DGR_RENDER_BWD_L(PPL_, U_, false); } while (0)
-        // the record staging follows the rule the forward applied to the same capacity (dgr_forward_render)
-        const int lz = g_lazy.load();
-        const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
+        // the record staging the forward chose (dgr_forward_render): only then does the sorted copy exist
+        const bool lazy = staging == DGR_STAGING_BY_ID;
         if (ppl == 1 && ub != 1 && !lazy && !g_rowsum.load()) {       // A/B: the default shape with the per-pixel step 2
 #define DGR_BWD_OLD_ render_bwd_kernel<1, 2, false, false>
             const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;

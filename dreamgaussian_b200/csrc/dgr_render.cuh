@@ -194,7 +194,7 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
     const bool costing = co.cost_acc != nullptr && PPL <= co.bwd_ppl;                 // forward sub-tiles nest in the backward's
     if (costing && blockIdx.x == 0 && threadIdx.x == 0) *co.cost_bpt = (unsigned)(8 / co.bwd_ppl);
     constexpr bool lazy = LAZY;
-    if (blockIdx.x == 0 && threadIdx.x == 0) *lazy_note = LAZY ? 1u : 0u;             // (for the record; the host picks the backward's variant by the same rule)
+    if (blockIdx.x == 0 && threadIdx.x == 0) *lazy_note = LAZY ? 1u : 0u;             // (for the record; the host hands its choice to the backward)
     const bool light = two_ended && (((blockIdx.x / (unsigned)sms) + (threadIdx.x >> 5)) & 1u);
     bool queue_phase = true;
     unsigned item = 0, empty_next = n_queue + warp_global;
@@ -405,7 +405,7 @@ render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
     ring_init(rg, rs, lane);
     // work list: the measured-cost classes of the forward (heaviest class first) when it grouped its costs for this sub-tile
     // shape, else every sub-tile of the non-empty tiles in population order
-    constexpr bool lazy = LAZY;                                      // the host picks the variant by the rule the forward used
+    constexpr bool lazy = LAZY;                                      // the host launches the variant its forward used
     (void)lazy_note;
     const bool by_cost = co.cost_acc != nullptr && __ldcg(co.cost_bpt) == (unsigned)ST::kPerTile;
     unsigned cum_end = 0;                                            // lane L: items in classes kCostClasses-1 .. kCostClasses-1-L

@@ -49,6 +49,7 @@ struct State {                       // what one forward leaves behind for its b
     Tensor geom, binning, image, radii;      // NOT the differentiable outputs: State -> output -> grad_fn -> ctx -> State would be an
                                              // uncollectable cycle through C++ reference counts (radii is non-differentiable: no grad_fn)
     int64_t capacity = 0, n_inst = 0;
+    int32_t staging = DGR_STAGING_SORTED;    // record staging the last stage-2 run chose (counts_host[3]): the backward's too
     int device = 0;
 };
 
@@ -157,7 +158,7 @@ forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modif
         rerun = DGR_FLAG_RERUN;
     }
     { std::lock_guard<std::mutex> lk(g_mu); g_hints[key] = Hint{std::max<int64_t>((int64_t)(n_inst * 1.25) + 4096, 65536), n_big > 0}; }
-    st->capacity = cap; st->n_inst = n_inst;
+    st->capacity = cap; st->n_inst = n_inst; st->staging = (int32_t)so.counts.data_ptr<int64_t>()[3];
     return {color, st->radii, depth, alpha, st};
 }
 
@@ -189,7 +190,7 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D),
                           reinterpret_cast<const DgrPeerPush *>(push_addr)};      // host struct kept alive by the caller (0 = none)
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
-    check(dgr_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->image.data_ptr(),
+    check(dgr_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
                        st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, stream));
     return g;
 }

@@ -167,8 +167,8 @@ def _stream_ptr(device):
 
 class ForwardState:
     """Everything one forward leaves behind for its backward (upstream: ctx + geom/binning/img buffers)."""
-    __slots__ = ("rs", "frame", "num_rendered", "capacity", "geom", "binning", "image", "radii", "alpha", "tensors", "fast",
-                 "stats_applied")
+    __slots__ = ("rs", "frame", "num_rendered", "capacity", "staging", "geom", "binning", "image", "radii", "alpha", "tensors",
+                 "fast", "stats_applied")
 
 
 def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, sh_rest=None, activations=False):
@@ -224,6 +224,7 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
     state = ForwardState()
     state.fast = None
     state.rs, state.frame, state.num_rendered, state.capacity = rs, fr, n_inst, cap
+    state.staging = int(n_host[3])                  # record staging of the last stage-2 run: its backward must use the same
     # alpha is a differentiable OUTPUT: storing it here would close the cycle state -> alpha -> grad_fn -> ctx -> state and leave
     # ~100 MB of scratch per call to the cyclic garbage collector (the C ABI's out_alpha argument is unused)
     state.geom, state.binning, state.image, state.radii, state.alpha = geom, binning, image, radii, None
@@ -269,7 +270,7 @@ def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2
                                      _ptr(d_rot), _ptr(d_cov), 1 if accumulate else 0, _ptr(d_sh_rest),
                                      *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), push_addr or None)
         _lib.check(lib.dgr_backward(ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(state.geom), _ptr(state.binning),
-                                    ctypes.c_uint64(state.capacity), _ptr(state.image), _ptr(state.radii), _ptr(state.alpha),
+                                    ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii), _ptr(state.alpha),
                                     ctypes.byref(gin), ctypes.byref(gout), _stream_ptr(dev)))
 
 

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define DGR_ABI_VERSION 4
+#define DGR_ABI_VERSION 5
 
 /* == GaussianRasterizationSettings, the 12-field NamedTuple built at gs_renderer.py:745-758 == */
 typedef struct DgrSettings {
@@ -138,9 +138,14 @@ int dgr_forward_preprocess(const DgrSettings *s, const DgrGaussians *g, void *ge
  *                No copy or event sits between the kernels then, so the whole forward chains with programmatic dependent
  *                launches (each kernel's prologue overlaps its predecessor's tail); count_ready_event is ignored.  If counts_host[0] > capacity_instances, or counts_host[1] > 0 without
  * DGR_FLAG_BIG_TILES, the call produced a memory-safe but wrong image: re-run stage 2 with corrected guesses and
- * DGR_FLAG_RERUN set. */
+ * DGR_FLAG_RERUN set.
+ * counts_host[3] is written by the host before the call returns (either protocol): the record staging this call chose for
+ * its render kernels (DGR_STAGING_SORTED or DGR_STAGING_BY_ID, see dgr_set_tuning bits 22-23).  The sorted record copy only
+ * exists in `binning` when it says DGR_STAGING_SORTED; the backward of this call must be given that value. */
 #define DGR_FLAG_BIG_TILES 1
 #define DGR_FLAG_RERUN 2      /* set when stage 2 is repeated for the same stage 1 (corrected guesses) */
+#define DGR_STAGING_SORTED 0  /* the sort kernel wrote a depth-sorted copy of the records; the render kernels stream it */
+#define DGR_STAGING_BY_ID 1   /* only the sorted Gaussian ids exist; the render kernels fetch every record by id */
 int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom, void *binning,
                        uint64_t capacity_instances, void *image, const DgrImages *out, int32_t flags,
                        uint64_t *counts_host, uint64_t ticket, void *count_ready_event, void *stream);
@@ -158,7 +163,9 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom, 
  *                each warp's 32 contiguous Gaussians through shared memory with bulk TMA (A/B switch; the staged path needs
  *                SH + scale / rotation inputs and 16-byte aligned base pointers and is otherwise not taken anyway)
  *   bit 26       step 2 of the backward render kernel in its per-pixel form (A/B switch; default sub-tile shape only)
- * the other bits are accepted and ignored. */
+ *   bit 28       per-tile depth sort with 2048 instead of 1024 buckets (A/B switch)
+ * the other bits are accepted and ignored.  The knobs may change between a forward and its backward: each call reads them when
+ * it launches, and the backward stages its records the way its forward did (counts_host[3] -> dgr_backward's `staging`). */
 int dgr_set_tuning(int ppl_fwd, int ppl_bwd, int tile_order);
 
 /* Thin cudaEvent wrappers so a host without the CUDA runtime headers (ctypes, cgo ...) can use the protocol above. */
@@ -167,11 +174,12 @@ int dgr_event_synchronize(void *event);
 void dgr_event_destroy(void *event);
 
 /* Backward of both stages.  geom / binning / image are the scratch buffers of the matching forward
- * (`capacity_instances` = the value stage 2 ran with); geom is also used as scratch for the per-Gaussian
+ * (`capacity_instances` = the value stage 2 ran with, `staging` = the counts_host[3] that call left: DGR_STAGING_SORTED or
+ * DGR_STAGING_BY_ID; when stage 2 was re-run, those of the last run); geom is also used as scratch for the per-Gaussian
  * reduction.  `out_alpha` is the alpha image the forward produced (accepted for signature parity with the
  * reference binding; the final transmittance is kept in `image` at full precision instead of 1 - alpha). */
 int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom, const void *binning,
-                 uint64_t capacity_instances, const void *image, const int32_t *radii, const float *out_alpha,
+                 uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii, const float *out_alpha,
                  const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream);
 
 /* Multi-GPU (view-sharded data parallelism, SURVEY.md §8e): all-reduce(sum) of the flat float32 gradient buffer over

@@ -75,8 +75,9 @@ def run_oracle(settings, inputs, grads=None, dtype=np.float64, eps=2e-5):
     return out
 
 
-def run_cuda(settings, inputs, grads=None, device="cuda"):
-    """The product path: GaussianRasterizer on CUDA tensors. Returns numpy outputs (+ grads)."""
+def run_cuda(settings, inputs, grads=None, device="cuda", before_backward=None):
+    """The product path: GaussianRasterizer on CUDA tensors. Returns numpy outputs (+ grads).  before_backward, if given, is
+    called between the forward and the backward (e.g. to change the tuning knobs in between)."""
     import torch
     from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
     t = lambda a: torch.tensor(np.asarray(a, np.float32), device=device)
@@ -95,6 +96,8 @@ def run_cuda(settings, inputs, grads=None, device="cuda"):
         loss = (color * t(gC)).sum() + (alpha * t(gA)).sum()
         if gD is not None:
             loss = loss + (depth * t(gD)).sum()
+        if before_backward is not None:
+            before_backward()
         loss.backward()
         g = {k: v.grad.detach().cpu().numpy() for k, v in tin.items()}
         g["means2D"] = means2D.grad.detach().cpu().numpy()
@@ -246,6 +249,54 @@ def compare_f32(cu, ref32):
                            or np.percentile(e, 99.9) > F32_GRAD_ATOL):
                 ok = False
     return ok, rep
+
+
+def oracles(settings, inputs, grads, f64=True):
+    """Both CPU oracle results of one case (float32 build, and float64 unless f64=False), to be reused for every CUDA run of it."""
+    return dict(f32=run_oracle(settings, inputs, grads, dtype=np.float32), f64=run_oracle(settings, inputs, grads) if f64 else None)
+
+
+def both_oracles(name, s, i, g, max_ambig_frac=MAX_AMBIG_FRAC, f64=True, refs=None, cu=None):
+    """The rule of the suite: the CUDA result must agree (a) with the float64 oracle on everything that oracle does not flag
+    as a decision a float32 implementation may take differently, and (b) with the float32 oracle with NO such exemption —
+    only float32 depth-key ties are set aside there.  refs: oracles() of the case (computed here when None); cu: the CUDA
+    result to judge (run here when None).  Returns the CUDA result."""
+    if refs is None:
+        refs = oracles(s, i, g, f64=f64)
+    if cu is None:
+        cu = run_cuda(s, i, g)
+    ok32, rep32 = compare_f32(cu, refs["f32"])
+    if refs["f64"] is not None:
+        ok64, rep64 = compare(cu, refs["f64"], max_ambig_frac=max_ambig_frac)
+    else:
+        ok64, rep64 = True, {}
+    report(name, vs_f64=rep64, vs_f32=rep32)
+    assert ok64, ("float64 oracle", rep64)
+    assert ok32, ("float32 oracle", rep32)
+    return cu
+
+
+DEFAULT_TUNING = (1, 1, 1)
+
+
+def set_tuning(word):
+    """dgr_set_tuning(ppl_fwd, ppl_bwd, bits) — process-wide until changed again."""
+    from dreamgaussian_b200 import _lib
+    _lib.check(_lib.load().dgr_set_tuning(*word))
+
+
+def run_tuned(word, fn, fast_host=True):
+    """fn() with the rasterizer tuned by `word` and the compiled (fast_host) or the ctypes host layer; the default tuning and
+    the compiled host layer are restored afterwards, whatever fn does."""
+    from dreamgaussian_b200 import rasterizer as R
+    try:
+        if R.set_fast_host(fast_host) != fast_host:
+            raise RuntimeError("the compiled host layer is not available")
+        set_tuning(word)
+        return fn()
+    finally:
+        set_tuning(DEFAULT_TUNING)
+        R.set_fast_host(True)
 
 
 def report(name, **reps):

@@ -18,7 +18,9 @@ def _declared_functions():
     return sorted(set(re.findall(r"\b(dgr_[a-z_0-9]+)\s*\(", src)))
 
 
-def test_library_builds_and_exports_every_declared_symbol():
+def test_library_builds_exports_every_declared_symbol_and_reports_the_header_abi_version():
+    """ABI 5: dgr_backward takes the record staging its forward reported in counts_host[3].  The library, the header and the
+    ctypes binding must agree on that version (the compiled host layer refuses to load otherwise)."""
     path = build.build()
     assert os.path.exists(path)
     lib = _lib.load()
@@ -27,7 +29,24 @@ def test_library_builds_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), "libdgr_b200.so does not export %s" % name
     assert set(_lib.EXPORTS) <= set(declared)
-    assert lib.dgr_abi_version() == _lib.ABI_VERSION == 4
+    header = open(os.path.join(ROOT, "include", "dgr_b200.h")).read()
+    assert int(re.search(r"#define DGR_ABI_VERSION (\d+)", header).group(1)) == lib.dgr_abi_version() == _lib.ABI_VERSION == 5
+
+
+def test_backward_rejects_a_record_staging_its_forward_cannot_have_reported():
+    """dgr_backward's `staging` is DGR_STAGING_SORTED (0) or DGR_STAGING_BY_ID (1), what dgr_forward_render left in
+    counts_host[3]; anything else fails with an error before any device work (the pointers here are never dereferenced)."""
+    import ctypes
+    lib = _lib.load()
+    buf = (ctypes.c_float * 64)()
+    p = ctypes.cast(buf, ctypes.c_void_p)
+    s = _lib.DgrSettings(16, 16, 0.5, 0.5, 1.0, 0, 0, 0, p, p, p, p)
+    g = _lib.DgrGaussians(1, 1, p, p, None, p, p, p, None, None, 0)
+    gin, gout = _lib.DgrImageGrads(p, None, None), _lib.DgrGaussianGrads()
+    for bad in (-1, 2, 7):
+        rc = lib.dgr_backward(ctypes.byref(s), ctypes.byref(g), p, p, ctypes.c_uint64(16), bad, p, p, None, ctypes.byref(gin),
+                              ctypes.byref(gout), None)
+        assert rc != 0 and b"staging" in lib.dgr_last_error(), bad
 
 
 def test_scratch_size_queries_need_no_gpu():

@@ -25,19 +25,7 @@ CASES = {
 }
 
 
-def both_oracles(name, s, i, g, max_ambig_frac=h.MAX_AMBIG_FRAC, f64=True):
-    """The rule of the suite: the CUDA result must agree (a) with the float64 oracle on everything that oracle does not flag
-    as a decision a float32 implementation may take differently, and (b) with the float32 oracle with NO such exemption —
-    only float32 depth-key ties are set aside there."""
-    cu = h.run_cuda(s, i, g)
-    ok32, rep32 = h.compare_f32(cu, h.run_oracle(s, i, g, dtype=np.float32))
-    if f64:
-        ok64, rep64 = h.compare(cu, h.run_oracle(s, i, g), max_ambig_frac=max_ambig_frac)
-    else:
-        ok64, rep64 = True, {}
-    h.report(name, vs_f64=rep64, vs_f32=rep32)
-    assert ok64, ("float64 oracle", rep64)
-    assert ok32, ("float32 oracle", rep32)
+both_oracles = h.both_oracles          # the rule of the suite (tests/helpers.py)
 
 
 @pytest.mark.parametrize("name", list(CASES))
@@ -157,20 +145,6 @@ def test_mark_visible_and_input_validation():
     a = R.GaussianRasterizer(rs)(means2D=torch.zeros_like(ti["means3D"]), **ti)[0]
     b = R.GaussianRasterizer(rs2)(means2D=torch.zeros_like(ti["means3D"]), **ti)[0]
     assert torch.equal(a, b)
-
-
-def test_forward_is_deterministic_and_tuning_independent():
-    s, i = h.make_case(P=8000, res=200, deg=2)
-    ti, rs = _torch_inputs(i), _settings(s)
-    lib = _lib.load()
-    outs = []
-    for tune in ((1, 2, 1), (1, 2, 1), (2, 1, 0), (4, 4, 1)):
-        _lib.check(lib.dgr_set_tuning(*tune))
-        outs.append([o.clone() for o in R.GaussianRasterizer(rs)(means2D=torch.zeros_like(ti["means3D"]), **ti)])
-    _lib.check(lib.dgr_set_tuning(1, 1, 1))          # the defaults
-    for o in outs[1:]:
-        for a, b in zip(outs[0], o):
-            assert torch.equal(a, b)          # bit-identical: per-pixel arithmetic does not depend on the launch shape
 
 
 @pytest.mark.parametrize("case", ["plain", "raw"])

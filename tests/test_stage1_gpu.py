@@ -98,10 +98,11 @@ def test_densify_compaction_kernels_reproduce_the_reference_methods():
     cpu.check_against(m, "after_reset_adam_", rtol=5e-6, atol=1e-7)
 
 
-@pytest.mark.parametrize("P,deg,screen", [(5000, 0, 1), (30011, 3, 0), (257, 1, 1), (1, 0, 1)])
+@pytest.mark.parametrize("P,deg,screen", [(5000, 0, 1), (30011, 3, 0), (257, 1, 1), (1, 0, 1), (262401, 1, 1)])
 def test_densify_compaction_equals_the_tensor_indexing_path(P, deg, screen):
     """Same decisions, same order, same values as the device-agnostic restatement (stage1.py, pinned on the CPU by the
-    reference's outputs) on random models, including the no-world-size-prune variant and tiny point counts."""
+    reference's outputs) on random models, including the no-world-size-prune variant and tiny point counts.  P = 262401 is
+    1026 blocks of 256: the one-CTA scan of the per-block counts (1024 threads) carries over into a second pass."""
     rng = np.random.default_rng(P)
     M = (deg + 1) ** 2
     init = dict(xyz=rng.normal(0, 0.3, (P, 3)), f_dc=rng.normal(0, 1, (P, 1, 3)), f_rest=rng.normal(0, 0.1, (P, M - 1, 3)),
