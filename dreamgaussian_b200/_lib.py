@@ -58,6 +58,19 @@ class DgrGaussianGrads(ctypes.Structure):
     ]
 
 
+class DgrViews(ctypes.Structure):
+    """Settings of a batched-camera call (include/dgr_b200.h): the array fields are device pointers."""
+    _fields_ = [
+        ("V", ctypes.c_int32), ("image_height", ctypes.c_int32), ("image_width", ctypes.c_int32),
+        ("scale_modifier", ctypes.c_float), ("sh_degree", ctypes.c_int32), ("debug", ctypes.c_int32),
+        ("tanfov", c_f32p), ("bg", c_f32p), ("viewmatrix", c_f32p), ("projmatrix", c_f32p), ("campos", c_f32p),
+    ]
+
+
+VIEWS_MAX = 64                       # DGR_VIEWS_MAX
+VIEWS_MAX_RECORDS = 2 ** 31 - 1      # DGR_VIEWS_MAX_RECORDS: V x P
+
+
 class DgrPeerPush(ctypes.Structure):
     _fields_ = [("world", ctypes.c_int32), ("rank", ctypes.c_int32), ("gaussians_per_owner", ctypes.c_int64),
                 ("delta_floats", ctypes.c_int64 * 16)]
@@ -68,6 +81,8 @@ EXPORTS = (
     "dgr_geom_bytes", "dgr_image_bytes", "dgr_binning_bytes",
     "dgr_forward_preprocess", "dgr_forward_render", "dgr_backward", "dgr_mark_visible", "dgr_debug_geom",
     "dgr_profile_enable", "dgr_profile_collect", "dgr_event_create", "dgr_event_synchronize", "dgr_event_destroy", "dgr_set_tuning", "dgr_peer_allreduce", "dgr_peer_flag_bytes", "dgr_peer_reduce_staged", "dgr_peer_push_flat", "dgr_knn_scratch_bytes", "dgr_dist_cuda2", "dgr_fields_scratch_bytes", "dgr_extract_fields", "dgr_adam_step", "dgr_densify_scratch_bytes", "dgr_densify_plan", "dgr_densify_apply",
+    "dgr_views_geom_bytes", "dgr_views_image_bytes", "dgr_views_binning_bytes", "dgr_views_forward_preprocess",
+    "dgr_views_forward_render", "dgr_views_backward",
 )
 
 _lib = None
@@ -149,6 +164,20 @@ def load():
     lib.dgr_profile_enable.argtypes = [ctypes.c_int]
     lib.dgr_profile_collect.restype = ctypes.c_int
     lib.dgr_profile_collect.argtypes = [ctypes.c_char_p, ctypes.c_size_t, vp, ctypes.c_int]
+    lib.dgr_views_geom_bytes.restype = ctypes.c_size_t
+    lib.dgr_views_geom_bytes.argtypes = [i32, i32, i32, i32]
+    lib.dgr_views_image_bytes.restype = ctypes.c_size_t
+    lib.dgr_views_image_bytes.argtypes = [i32, i32, i32]
+    lib.dgr_views_binning_bytes.restype = ctypes.c_size_t
+    lib.dgr_views_binning_bytes.argtypes = [u64, i32, i32, i32]
+    lib.dgr_views_forward_preprocess.restype = ctypes.c_int
+    lib.dgr_views_forward_preprocess.argtypes = [ctypes.POINTER(DgrViews), ctypes.POINTER(DgrGaussians), vp, vp, vp, vp]
+    lib.dgr_views_forward_render.restype = ctypes.c_int
+    lib.dgr_views_forward_render.argtypes = [ctypes.POINTER(DgrViews), ctypes.POINTER(DgrGaussians), vp, vp, u64, vp,
+                                             ctypes.POINTER(DgrImages), i32, vp, u64, vp, vp]
+    lib.dgr_views_backward.restype = ctypes.c_int
+    lib.dgr_views_backward.argtypes = [ctypes.POINTER(DgrViews), ctypes.POINTER(DgrGaussians), vp, vp, u64, i32, vp, vp,
+                                       ctypes.POINTER(DgrImageGrads), ctypes.POINTER(DgrGaussianGrads), vp]
     if lib.dgr_abi_version() != ABI_VERSION:
         raise RuntimeError("libdgr_b200.so ABI version mismatch")
     _lib = lib

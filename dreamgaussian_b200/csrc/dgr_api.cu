@@ -282,6 +282,7 @@ DevInfo *dev_info() {
     int l2 = 0;
     if (cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) == cudaSuccess && l2 > 0) d.l2_bytes = (size_t)l2;
     cudaError_t e = cudaFuncSetAttribute(emit_instances_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTileSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(emit_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTileSmem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tile_sort_gather_kernel<kSortSmallBuckets>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmS::bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tile_sort_gather_kernel<kSortSmallBucketsFine>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmSF::bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tile_sort_gather_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmB::bytes);
@@ -591,6 +592,273 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
     DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, st));
     return 0;
 }
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Batched cameras (include/dgr_b200.h, DgrViews): one cloud, V same-size views.  Same pipeline as the single-view call on a
+// global tile space (tile v T + local tile) and V x P records (record v P + g).
+// ---------------------------------------------------------------------------------------------------------------------------
+namespace {
+int check_views(const DgrViews *s) {
+    if (!s) return fail(-1, "views settings is NULL");
+    if (s->V < 1 || s->V > DGR_VIEWS_MAX) return fail(-3, "views: V must be 1..64");
+    if (s->image_height <= 0 || s->image_width <= 0) return fail(-1, "image size must be positive");
+    if (s->image_height > 65535 || s->image_width > 65535) return fail(-1, "image size above 65535 not supported");
+    if (s->sh_degree < 0 || s->sh_degree > 3) return fail(-1, "sh_degree must be 0..3");
+    const size_t tiles = (size_t)((s->image_width + kTile - 1) / kTile) * (size_t)((s->image_height + kTile - 1) / kTile) * (size_t)s->V;
+    if (tiles * 4 > kMaxTileSmem) return fail(-3, "views: V x tiles per view above 51200 (16x16 tiles) not supported");
+    if (!s->tanfov || !s->bg || !s->viewmatrix || !s->projmatrix || !s->campos)
+        return fail(-1, "views: tanfov / bg / viewmatrix / projmatrix / campos must not be NULL");
+    return 0;
+}
+int check_views_gaussians(const DgrViews *s, const DgrGaussians *g) {
+    if (!g) return fail(-1, "gaussians is NULL");
+    if (g->P < 0) return fail(-1, "P < 0");
+    if ((long long)s->V * (long long)g->P > DGR_VIEWS_MAX_RECORDS) return fail(-3, "views: V x P above 2^31 - 1 records not supported");
+    if (g->P == 0) return 0;
+    if (g->colors_precomp || g->cov3D_precomp)
+        return fail(-2, "views: precomputed colours / cov3D are not supported by the batched call (SH + scale / rotation only)");
+    if (!g->shs || !g->scales || !g->rotations || !g->means3D || !g->opacities)
+        return fail(-1, "views: means3D / shs / opacities / scales / rotations must not be NULL");
+    if (g->activations && g->M > 1 && !g->shs_rest) return fail(-2, "activations: shs_rest (_features_rest) is NULL but M > 1");
+    const int nb = (s->sh_degree + 1) * (s->sh_degree + 1);
+    if (g->M < nb) return fail(-1, "shs has fewer coefficients than sh_degree needs");
+    if (g->M > 16) return fail(-1, "shs with more than 16 coefficients per channel not supported");
+    return 0;
+}
+
+constexpr size_t kViewsFwdStaticSmem = (size_t)kMaxViews * (sizeof(FrameConsts) + sizeof(float2)) + (kPreThreads / 32) * 8;
+
+template <int DEG, bool RAW>
+void launch_views_pre_fwd(const DgrViews *s, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L, int tiles_view,
+                          unsigned *tile_count, cudaStream_t st) {
+    unsigned *run_matrix = reinterpret_cast<unsigned *>(geom + L.off_runs);
+    const size_t hist = (size_t)L.tiles * 4;
+    // staged path: [tile histogram of the batch | 8 warps x 32 x (44 + 12 M) bytes], when it fits next to the cameras
+    const size_t stage_off = align_up(hist, 128);
+    const size_t smem_st = stage_off + (size_t)(kPreThreads / 32) * stage_warp_floats(g->M) * 4;
+    const bool staged = g_stage_fwd.load() && stage_inputs_ok(g, RAW) && smem_st + kViewsFwdStaticSmem + 1024 <= kMaxKernelSmem;
+    const size_t smem = staged ? smem_st : hist;
+#define DGR_VIEWS_PRE_FWD(STG_)                                                                                                   \
+    do {                                                                                                                         \
+        if (smem + kViewsFwdStaticSmem > 48 * 1024)          /* the cameras' static shared memory counts against the 48 KB */    \
+            cudaFuncSetAttribute(preprocess_views_fwd_kernel<DEG, RAW, STG_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        launch_k(preprocess_views_fwd_kernel<DEG, RAW, STG_>, dim3(L.nblocks), dim3(kPreThreads), smem, st, false, g->P, g->M, s->V,   \
+                 s->image_height, s->image_width, s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos, g->means3D,   \
+                 g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, radii, reinterpret_cast<Rec *>(geom + L.off_rec),          \
+                 reinterpret_cast<unsigned *>(geom + L.off_touched), tile_count, run_matrix, tiles_view, L.iters, (int)stage_off);     \
+    } while (0)
+    if (staged) DGR_VIEWS_PRE_FWD(true); else DGR_VIEWS_PRE_FWD(false);
+#undef DGR_VIEWS_PRE_FWD
+}
+
+template <int DEG, bool RAW>
+void launch_views_pre_bwd(const DgrViews *s, const DgrGaussians *g, const int *radii, const unsigned *touched, const float *grad_rec,
+                          const DgrGaussianGrads *o, cudaStream_t st) {
+    launch_k(preprocess_views_bwd_kernel<DEG, RAW>, dim3((g->P + kPreThreads - 1) / kPreThreads), dim3(kPreThreads), 0, st, true,
+             g->P, g->M, s->V, s->image_height, s->image_width, s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos,
+             g->means3D, g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, radii, touched, grad_rec, o->dL_dmeans3D,
+             o->dL_dmeans2D, o->dL_dshs, o->dL_dopacities, o->dL_dscales, o->dL_drotations, o->dL_dshs_rest, o->accumulate);
+}
+
+#define DGR_VIEWS_DISPATCH(FN, ...)                                                                        \
+    do {                                                                                                   \
+        if (g->activations) switch (s->sh_degree) {                                                        \
+            case 0: FN<0, true>(__VA_ARGS__); break;                                                       \
+            case 1: FN<1, true>(__VA_ARGS__); break;                                                       \
+            case 2: FN<2, true>(__VA_ARGS__); break;                                                       \
+            default: FN<3, true>(__VA_ARGS__); break;                                                      \
+        }                                                                                                  \
+        else switch (s->sh_degree) {                                                                       \
+            case 0: FN<0, false>(__VA_ARGS__); break;                                                      \
+            case 1: FN<1, false>(__VA_ARGS__); break;                                                      \
+            case 2: FN<2, false>(__VA_ARGS__); break;                                                      \
+            default: FN<3, false>(__VA_ARGS__); break;                                                     \
+        }                                                                                                  \
+    } while (0)
+}  // namespace
+
+extern "C" {
+
+size_t dgr_views_geom_bytes(int32_t V, int32_t P, int32_t H, int32_t W) { return GeomLayout(P, H, W, V > 0 ? V : 1).total; }
+size_t dgr_views_image_bytes(int32_t V, int32_t H, int32_t W) { return ImageLayout(H, W, V > 0 ? V : 1).total; }
+size_t dgr_views_binning_bytes(uint64_t cap, int32_t V, int32_t H, int32_t W) { (void)V; (void)H; (void)W; return BinningLayout(cap).total; }
+
+int dgr_views_forward_preprocess(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
+    NvtxRange nvtx_("dgr_views_forward_preprocess");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    char *geom = (char *)geom_v, *image = (char *)image_v;
+    if (!geom || !image) return fail(-1, "geom / image scratch is NULL");
+    if (g->P > 0 && !radii) return fail(-1, "radii is NULL");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H = s->image_height, W = s->image_width;
+    GeomLayout L(g->P, H, W, s->V);
+    ImageLayout IL(H, W, s->V);
+    const int tiles_view = IL.gx * IL.gy;
+    DGR_CUDA(cudaMemsetAsync(image + IL.off_work, 0, (IL.off_cost - IL.off_work) + (size_t)L.tiles * 8 * 4, st));
+    if (g->P > 0)
+        DGR_KERNEL("preprocess_views_fwd", st, s->debug,
+                   DGR_VIEWS_DISPATCH(launch_views_pre_fwd, s, g, radii, geom, L, tiles_view, reinterpret_cast<unsigned *>(image + IL.off_count), st));
+    return 0;
+}
+
+int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                             void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                             void *count_ready_event, void *stream) {
+    NvtxRange nvtx_("dgr_views_forward_render");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    if (!geom_v || !image_v || !out) return fail(-1, "NULL argument");
+    if (!out->color || !out->depth || !out->alpha) return fail(-1, "output images must not be NULL");
+    if (capacity > 0 && !binning_v) return fail(-1, "binning scratch is NULL");
+    if (capacity >= 0xffffffffull) return fail(-3, "capacity above 2^32-1 tile instances not supported");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *geom = (char *)geom_v, *binning = (char *)binning_v, *image = (char *)image_v;
+    const int H = s->image_height, W = s->image_width;
+    GeomLayout GL(g->P, H, W, s->V);
+    ImageLayout IL(H, W, s->V);
+    BinningLayout BL(capacity);
+    const int tiles_view = IL.gx * IL.gy, tiles = tiles_view * s->V;
+    uint2 *ranges = reinterpret_cast<uint2 *>(image + IL.off_ranges);
+    unsigned *tile_count = reinterpret_cast<unsigned *>(image + IL.off_count);
+    const unsigned *run_matrix = reinterpret_cast<const unsigned *>(geom + GL.off_runs);
+    GeomHeader *hdr = reinterpret_cast<GeomHeader *>(geom);
+    const Rec *rec = reinterpret_cast<const Rec *>(geom + GL.off_rec);
+    unsigned long long *keys = binning ? reinterpret_cast<unsigned long long *>(binning + BL.off_keys) : nullptr;
+    unsigned *ids = binning ? reinterpret_cast<unsigned *>(binning + BL.off_ids) : nullptr;
+    Rec *recs = binning ? reinterpret_cast<Rec *>(binning + BL.off_rec) : nullptr;
+    unsigned *tile_order = reinterpret_cast<unsigned *>(image + IL.off_order);
+    unsigned *big_list = reinterpret_cast<unsigned *>(image + IL.off_biglist);
+    TileWork *work = reinterpret_cast<TileWork *>(image + IL.off_work);
+    DevInfo *dv = dev_info();
+    if (!dv) return -1;
+    if (flags & DGR_FLAG_RERUN) {
+        DGR_CUDA(cudaMemsetAsync(image + IL.off_cost, 0, (size_t)tiles * 8 * 4, st));
+        DGR_CUDA(cudaMemsetAsync(reinterpret_cast<char *>(work) + offsetof(TileWork, cost_bpt), 0, sizeof(TileWork) - offsetof(TileWork, cost_bpt), st));
+    }
+    {
+        const int nb = (g->P > 0 && capacity > 0) ? GL.nblocks : 0;
+        DGR_KERNEL("emit_views", st, s->debug,
+                   launch_k(emit_views_kernel, dim3(nb + 1), dim3(kPreThreads), (size_t)tiles * 4, st, !(flags & DGR_FLAG_RERUN), g->P, s->V, IL.gx,
+                            tiles_view, GL.iters, nb, rec, reinterpret_cast<const unsigned *>(geom + GL.off_touched), (const unsigned *)tile_count,
+                            (unsigned long long)capacity, run_matrix, keys, ranges, hdr, tile_order, reinterpret_cast<uint2 *>(image + IL.off_oranges),
+                            work, big_list, (volatile unsigned long long *)(ticket ? counts_host : nullptr), (unsigned long long)ticket));
+    }
+    if (!ticket) {
+        if (counts_host) DGR_CUDA(cudaMemcpyAsync(counts_host, geom, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        if (count_ready_event) DGR_CUDA(cudaEventRecord((cudaEvent_t)count_ready_event, st));
+    }
+    // record staging: the rule of dgr_forward_render, reported to the caller for the backward
+    const int lz = g_lazy.load();
+    const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
+    if (counts_host) counts_host[3] = lazy ? DGR_STAGING_BY_ID : DGR_STAGING_SORTED;
+    if (g->P > 0 && capacity > 0) {
+        if (g_sort_fine.load()) {
+            const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBucketsFine>, kSortSmallThreads, SmSF::bytes));
+            DGR_KERNEL("tile_sort_gather", st, s->debug,
+                       launch_k(tile_sort_gather_kernel<kSortSmallBucketsFine>, dim3(sort_grid), dim3(kSortSmallThreads), SmSF::bytes, st, true, (const TileWork *)work,
+                                reinterpret_cast<const uint2 *>(image + IL.off_oranges), keys, rec, ids, recs, lazy ? 0 : 1));
+        } else {
+            const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBuckets>, kSortSmallThreads, SmS::bytes));
+            DGR_KERNEL("tile_sort_gather", st, s->debug,
+                       launch_k(tile_sort_gather_kernel<kSortSmallBuckets>, dim3(sort_grid), dim3(kSortSmallThreads), SmS::bytes, st, true, (const TileWork *)work,
+                                reinterpret_cast<const uint2 *>(image + IL.off_oranges), keys, rec, ids, recs, lazy ? 0 : 1));
+        }
+        if (flags & DGR_FLAG_BIG_TILES)
+            DGR_KERNEL("tile_sort_gather_big", st, s->debug,
+                       launch_k(tile_sort_gather_big_kernel, dim3(dv->big_grid), dim3(kSortBigThreads), SmB::bytes, st, true, (const TileWork *)work,
+                                (const unsigned *)big_list, (const uint2 *)ranges, keys, rec, ids, recs, lazy ? 0 : 1));
+    }
+    CostOrder co{};
+    if (g_cost_order.load()) {
+        co.cost_acc = reinterpret_cast<unsigned *>(image + IL.off_cost); co.cls_count = work->cls_count;
+        co.cls_items = reinterpret_cast<unsigned *>(image + IL.off_clsitems); co.cost_bpt = &work->cost_bpt;
+        co.tiles = tiles; co.bwd_ppl = 1;                       // the batched backward's 8x4 sub-tiles
+    }
+#define DGR_VIEWS_FWD(L_)                                                                                                   \
+    do {                                                                                                                   \
+        const int items_ = tiles * SubTile<1>::kPerTile;                                                                   \
+        int grid_ = min(persistent_grid(dv, render_views_fwd_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
+        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                                          \
+        DGR_KERNEL("render_views_fwd", st, s->debug,                                                                       \
+                   launch_k(render_views_fwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, H, W, IL.gx, \
+                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),          \
+                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
+                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids, s->bg, out->color, out->depth, out->alpha, \
+                            reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT), tiles_view)); \
+    } while (0)
+    if (lazy) DGR_VIEWS_FWD(true); else DGR_VIEWS_FWD(false);
+#undef DGR_VIEWS_FWD
+    return 0;
+}
+
+int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                       const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
+    NvtxRange nvtx_("dgr_views_backward");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
+    if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
+        return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
+    if (gout->xyz_gradient_accum || gout->denom || gout->max_radii2D)
+        return fail(-2, "views: the fused densification statistics are not supported by the batched call");
+    if (gout->push) return fail(-2, "views: DgrPeerPush is not supported by the batched call");
+    if (gout->dL_dcolors_precomp || gout->dL_dcov3D_precomp)
+        return fail(-2, "views: precomputed colours / cov3D are not supported by the batched call (SH + scale / rotation only)");
+    if (g->P == 0) return 0;
+    if (!radii) return fail(-1, "radii is NULL");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *geom = (char *)geom_v;
+    const char *binning = (const char *)binning_v, *image = (const char *)image_v;
+    const int H = s->image_height, W = s->image_width;
+    GeomLayout GL(g->P, H, W, s->V);
+    ImageLayout IL(H, W, s->V);
+    BinningLayout BL(capacity);
+    const int tiles_view = IL.gx * IL.gy, tiles = tiles_view * s->V;
+    float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
+    DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * s->V * kGradRecFloats * 4, st));
+    if (binning && capacity > 0) {
+        DevInfo *dv = dev_info();
+        if (!dv) return -1;
+        const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
+        unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
+        CostOrder co{};
+        if (g_cost_order.load()) {
+            TileWork *wk = const_cast<TileWork *>(work);
+            co.cost_acc = const_cast<unsigned *>(reinterpret_cast<const unsigned *>(image + IL.off_cost)); co.cls_count = wk->cls_count;
+            co.cls_items = const_cast<unsigned *>(reinterpret_cast<const unsigned *>(image + IL.off_clsitems)); co.cost_bpt = &wk->cost_bpt;
+            co.tiles = tiles; co.bwd_ppl = 1;
+        }
+        const bool lazy = staging == DGR_STAGING_BY_ID;
+#define DGR_VIEWS_BWD(L_)                                                                                                       \
+    do {                                                                                                                       \
+        const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;                                                                \
+        int grid_ = min(persistent_grid(dv, render_views_bwd_kernel<L_>, kRenderThreads, smem_),                               \
+                        (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);                                     \
+        if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);                                              \
+        DGR_KERNEL("render_views_bwd", st, s->debug,                                                                           \
+                   launch_k(render_views_bwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, H, W, IL.gx, \
+                            reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co, \
+                            reinterpret_cast<const uint2 *>(image + IL.off_oranges),                                           \
+                            reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec), \
+                            (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),             \
+                            s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),                                     \
+                            reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, \
+                            grad_rec, tiles_view));                                                                            \
+    } while (0)
+        if (lazy) DGR_VIEWS_BWD(true); else DGR_VIEWS_BWD(false);
+#undef DGR_VIEWS_BWD
+    }
+    DGR_KERNEL("preprocess_views_bwd", st, s->debug,
+               DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, st));
+    return 0;
+}
+
+}  // extern "C"
+
+extern "C" {
 
 #include "dgr_collective_api.cuh"      // dgr_peer_*: the multi-GPU entry points (not part of the single-GPU step)
 

@@ -196,6 +196,72 @@ tile_meta_cta(int tiles, const unsigned *__restrict__ tile_count, unsigned long 
     }
 }
 
+// Instance emission, first half: this block's write cursor of every tile = start of the tile's range (exclusive scan of the
+// per-tile totals) + where the preprocess kernel's reservation put this block inside the tile (its run-matrix row).
+__device__ __forceinline__ void emit_block_cursors(int tiles, const unsigned *__restrict__ tile_count, unsigned long long cap,
+                                                   const unsigned *__restrict__ run_matrix, unsigned *s_off, unsigned long long *s_part) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    // range starts: exclusive scan of the per-tile totals.  Warp w owns the contiguous tile range [w R, (w + 1) R); its lanes
+    // read 32 consecutive tiles at a time (coalesced, several loads in flight): pass 1 sums the range, pass 2 (after the
+    // warp bases are known) scans it and adds the block's run-matrix row.
+    constexpr int NW = kPreThreads / 32;
+    const int R = ((tiles + NW - 1) / NW + 31) / 32 * 32;
+    const int w_lo = min(tiles, warp * R), w_hi = min(tiles, w_lo + R);
+    unsigned long long sum = 0;
+#pragma unroll 4
+    for (int t = w_lo + lane; t < w_hi; t += 32) sum += __ldcg(tile_count + t);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (lane == 0) s_part[warp] = sum;
+    __syncthreads();
+    unsigned long long run = 0;
+    for (int w = 0; w < warp; w++) run += s_part[w];
+    const unsigned *row = run_matrix + (size_t)blockIdx.x * tiles;
+    // (the totals and run-matrix entries of kE 32-tile pieces are requested before the first of them is scanned: the scans form
+    //  a dependent chain through `run`, and one L2 round trip per piece would otherwise sit in front of every link of it)
+    constexpr int kE = 4;
+    for (int t0 = w_lo; t0 < w_hi; t0 += 32 * kE) {
+        unsigned cj[kE], rj[kE];
+#pragma unroll
+        for (int j = 0; j < kE; j++) {
+            const int t = t0 + 32 * j + lane;
+            cj[j] = t < w_hi ? __ldcg(tile_count + t) : 0u;
+            rj[j] = t < w_hi ? __ldcg(row + t) : 0u;
+        }
+#pragma unroll
+        for (int j = 0; j < kE; j++) {
+            if (t0 + 32 * j < w_hi) {                                     // warp-uniform
+                const int t = t0 + 32 * j + lane;
+                const unsigned c = cj[j];
+                unsigned inc = c;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) { const unsigned n = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += n; }
+                const unsigned long long start = run + (inc - c);
+                if (t < w_hi) s_off[t] = (unsigned)(start < cap ? start : cap) + rj[j];
+                run += __shfl_sync(0xffffffffu, inc, 31);
+            }
+        }
+    }
+    __syncthreads();
+}
+
+// Instance emission, second half: one Gaussian's `cnt` instances (the tiles of its packed pixel AABB ax / ay, offset by tile0)
+// at the block's tile cursors: ONE shared-memory atomic and one 8-byte store per instance.  Positions at or beyond the
+// capacity are dropped.
+__device__ __forceinline__ void emit_keys(unsigned long long key, unsigned ax, unsigned ay, int gx, int tile0, int cnt, unsigned *s_off,
+                                          unsigned long long *__restrict__ keys, unsigned cap32) {
+    const int tx0 = (int)(ax & 0xffffu) >> 4, tw = ((int)(ax >> 16) >> 4) - tx0 + 1;
+    const int ty0 = (int)(ay & 0xffffu) >> 4;
+    int x = 0, t = tile0 + ty0 * gx + tx0;
+#pragma unroll 4
+    for (int i = 0; i < cnt; i++) {
+        const unsigned pos = atomicAdd(&s_off[t], 1u);
+        if (pos < cap32) keys[pos] = key;                             // beyond the instance capacity: dropped
+        x++; t++;
+        if (x == tw) { x = 0; t += gx - tw; }
+    }
+}
+
 // Instance emission, same block <-> Gaussian mapping as the preprocess kernel; grid = nblocks + 1.
 //   blocks 0 .. nblocks-1:  the block scans the per-tile totals itself for the range starts (every thread owns a run of
 //     consecutive tiles; the totals are 4 B x tiles, L2-resident), adds its row of the run matrix (where the preprocess
@@ -277,6 +343,40 @@ emit_instances_kernel(int P, int gx, int tiles, int gpb_iters, int nblocks, cons
             if (pos < cap32) keys[pos] = key;                             // beyond the instance capacity: dropped
             x++; t++;
             if (x == tw) { x = 0; t += gx - tw; }
+        }
+    }
+}
+
+// Batched emission (dgr_views_*): the same block <-> Gaussian mapping as preprocess_views_fwd_kernel; each Gaussian appends the
+// instances of all its views: key = depth bits << 32 | record r = v P + g, in the tiles v T + local tile.  The metadata block
+// covers the V T tiles of the batch.
+__global__ void __launch_bounds__(kPreThreads)
+emit_views_kernel(int P, int V, int gx, int tiles_view, int gpb_iters, int nblocks, const Rec *__restrict__ rec, const unsigned *__restrict__ touched,
+                  const unsigned *__restrict__ tile_count, unsigned long long cap, const unsigned *__restrict__ run_matrix,
+                  unsigned long long *__restrict__ keys, uint2 *__restrict__ ranges, GeomHeader *__restrict__ hdr,
+                  unsigned *__restrict__ tile_order, uint2 *__restrict__ order_ranges, TileWork *__restrict__ work,
+                  unsigned *__restrict__ big_list, volatile unsigned long long *counts_host, unsigned long long ticket) {
+    extern __shared__ unsigned s_off[];
+    __shared__ unsigned long long s_part[kPreThreads / 32];
+    pdl_trigger();
+    pdl_wait();
+    const int tiles = V * tiles_view;
+    if ((int)blockIdx.x == nblocks) {
+        tile_meta_cta<kPreThreads>(tiles, tile_count, cap, ranges, hdr, tile_order, order_ranges, work, big_list, counts_host, ticket);
+        return;
+    }
+    emit_block_cursors(tiles, tile_count, cap, run_matrix, s_off, s_part);
+    const unsigned cap32 = (unsigned)cap;
+    for (int it = 0; it < gpb_iters; it++) {
+        const int g = (int)((blockIdx.x * gpb_iters + it) * kPreThreads + threadIdx.x);
+        if (g >= P) continue;
+        for (int v = 0; v < V; v++) {
+            const unsigned r = (unsigned)v * (unsigned)P + (unsigned)g;
+            const int cnt = (int)(__ldg(touched + r) & 0x1fffffffu);
+            if (cnt == 0) continue;
+            const float4 q1 = __ldg(&rec[r].q1);
+            const unsigned long long key = ((unsigned long long)__float_as_uint(q1.z) << 32) | r;
+            emit_keys(key, __float_as_uint(q1.w), __float_as_uint(__ldg(&rec[r].q2.w)), gx, v * tiles_view, cnt, s_off, keys, cap32);
         }
     }
 }

@@ -63,20 +63,24 @@ __host__ __device__ inline int choose_gpb_iters(int P, int tiles) {
 // geom scratch: [header 256][rec 48 x P][touched u32 x P][backward work counter 256][moments 48 x P (backward)]
 //               [run matrix u32 x blocks x tiles: where block b's instances start inside tile t's range]
 //               (the backward zeroes counter + moments with ONE memset)
+// A batch of V views of one cloud (dgr_views_*) keeps V x P records (record r = v P + g) and V x tiles-per-view tiles
+// (global tile v T + local tile); the blocks still cover the P Gaussians, so the run matrix is blocks x V T.
 struct GeomLayout {
     size_t off_rec, off_touched, off_bwdwork, off_gradrec, off_runs, total;
     int tiles, iters, nblocks;
-    __host__ __device__ GeomLayout(int P, int H, int W) {
+    __host__ __device__ GeomLayout(int P, int H, int W, int V = 1) {
         size_t Pn = P > 0 ? (size_t)P : 1;
+        const size_t Rn = Pn * (size_t)V;
         tiles = ((W + kTile - 1) / kTile) * ((H + kTile - 1) / kTile);
         if (tiles < 1) tiles = 1;
+        tiles *= V;
         iters = choose_gpb_iters(P, tiles);
         nblocks = (int)((Pn + (size_t)kPreThreads * iters - 1) / ((size_t)kPreThreads * iters));
         size_t o = 256;
-        off_rec = o;     o = align_up(o + Pn * sizeof(Rec), 256);
-        off_touched = o; o = align_up(o + Pn * 4, 256);
+        off_rec = o;     o = align_up(o + Rn * sizeof(Rec), 256);
+        off_touched = o; o = align_up(o + Rn * 4, 256);
         off_bwdwork = o; o += 256;
-        off_gradrec = o; o = align_up(o + Pn * kGradRecFloats * 4, 256);
+        off_gradrec = o; o = align_up(o + Rn * kGradRecFloats * 4, 256);
         off_runs = o;    o = align_up(o + (size_t)nblocks * tiles * 4, 256);
         total = o;
     }
@@ -88,13 +92,15 @@ constexpr int kCostClasses = 32;         // log-scale classes of the measured fo
 //                [big_list u32 x tiles][n_contrib u32 x HW][final_T f32 x HW]
 //                ... [cost accumulators u32 x 8 tiles] ... [cost-class item lists u32 x 32 x 8 tiles]
 // (work, tile_count and the cost accumulators are adjacent: the forward zeroes them with ONE memset before the preprocess kernel)
+// V views (dgr_views_*): every per-tile array covers V x tiles-per-view tiles and n_contrib / final_T are [V, H, W].
 struct ImageLayout {
     size_t off_ranges, off_oranges, off_count, off_cost, off_order, off_biglist, off_work, off_ncontrib, off_finalT, off_clsitems, total;
     int gx, gy;
-    __host__ __device__ ImageLayout(int H, int W) {
+    __host__ __device__ ImageLayout(int H, int W, int V = 1) {
         gx = (W + kTile - 1) / kTile; gy = (H + kTile - 1) / kTile;
         size_t tiles = (size_t)gx * gy; if (tiles < 1) tiles = 1;
         size_t hw = (size_t)H * W; if (hw < 1) hw = 1;
+        tiles *= (size_t)V; hw *= (size_t)V;
         size_t o = 0;
         off_work = o;     o = align_up(o + 256, 256);
         off_count = o;    o = align_up(o + tiles * 4, 256);

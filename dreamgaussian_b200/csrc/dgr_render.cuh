@@ -166,15 +166,18 @@ struct CostOrder {                       // image scratch pieces (all may be NUL
 // only the short T / colour update runs in sequence.  Same per-pixel operation order for every U: bit-identical images.
 // One-pixel-per-lane variants are held to 64 registers (8 CTAs per SM): measured 4-5 us per step at 100k / 800^2 against the
 // 72 registers ptxas picks on its own (A/B in profiles/r2_ab_variants.log).
-template <int PPL, int U, bool LAZY>
-__global__ void __launch_bounds__(kRenderThreads, PPL == 1 ? 8 : 1)
-render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+//
+// VIEWS: a batch of V same-size views (dgr_views_forward_render).  Tiles are numbered v T + local tile (T = tiles_view), every
+// view has its own background (bg [V,3]) and its own slices of the [V, ...] images; the records are those of the batch.
+template <int PPL, int U, bool LAZY, bool VIEWS>
+__device__ __forceinline__ void
+render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
                   const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
                   int two_ended, int sms, CostOrder co, unsigned *__restrict__ lazy_note,
                   const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
                   const float *__restrict__ bg, float *__restrict__ out_color,
                   float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
-                  float *__restrict__ final_T) {
+                  float *__restrict__ final_T, int tiles_view) {
     using ST = SubTile<PPL>;
     __shared__ WarpRing rings[kRenderWarps];
     const int lane = threadIdx.x & 31;
@@ -182,7 +185,7 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
     RingState rs;
     pdl_trigger();
     ring_init(rg, rs, lane);
-    const float b0 = __ldg(bg), b1 = __ldg(bg + 1), b2 = __ldg(bg + 2);
+    const float b0 = VIEWS ? 0.f : __ldg(bg), b1 = VIEWS ? 0.f : __ldg(bg + 1), b2 = VIEWS ? 0.f : __ldg(bg + 2);    // VIEWS: per item
     const size_t HW = (size_t)H * W;
     pdl_wait();                          // sorted records, ranges, order, work counter
 
@@ -219,7 +222,8 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
         const unsigned ot = item / ST::kPerTile;
         const int tile = (int)__ldcg(tile_order + ot), sub = (int)(item % ST::kPerTile);
         const uint2 range = __ldcg(order_ranges + ot);
-        const int tx = tile % gx, ty = tile / gx;
+        const int v = VIEWS ? tile / tiles_view : 0, lt = VIEWS ? tile - v * tiles_view : tile;
+        const int tx = lt % gx, ty = lt / gx;
         const int n = (int)(range.y - range.x);
         const int nchunks = (n + kChunk - 1) / kChunk;
         const Rec *src = rec_sorted + range.x;
@@ -321,6 +325,25 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
         // never move on (or leave) with a bulk copy in flight into this warp's ring
         for (int c = rs.waited; c < rs.issued; c++) ring_wait(rg, rs, c);
 
+        if constexpr (VIEWS) {              // view v's background and slices of the [V, ...] images
+            const float vb0 = __ldg(bg + 3 * v), vb1 = __ldg(bg + 3 * v + 1), vb2 = __ldg(bg + 3 * v + 2);
+            const size_t vb = (size_t)v * HW;
+            float *oc = out_color + 3 * vb, *od = out_depth + vb, *oa = out_alpha + vb, *fT = final_T + vb;
+            unsigned *nc = n_contrib + vb;
+#pragma unroll
+            for (int p = 0; p < PPL; p++) {
+                if (inside[p]) {
+                    const size_t pix = (size_t)ST::py(wy0, lane, p) * W + ST::px(wx0, lane, p);
+                    oc[pix] = C0[p] + T[p] * vb0;
+                    oc[HW + pix] = C1[p] + T[p] * vb1;
+                    oc[2 * HW + pix] = C2[p] + T[p] * vb2;
+                    od[pix] = D[p];
+                    oa[pix] = 1.f - T[p];
+                    nc[pix] = last[p];
+                    fT[pix] = T[p];
+                }
+            }
+        } else {
 #pragma unroll
         for (int p = 0; p < PPL; p++) {
             if (inside[p]) {
@@ -333,6 +356,7 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
                 n_contrib[pix] = last[p];
                 final_T[pix] = T[p];
             }
+        }
         }
         if (costing && n > 0) {
             // this forward item's share of its backward item's cost; whoever completes the backward item files it under its class
@@ -363,6 +387,31 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
     }
 }
 
+template <int PPL, int U, bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads, PPL == 1 ? 8 : 1)
+render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+                  const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
+                  int two_ended, int sms, CostOrder co, unsigned *__restrict__ lazy_note,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
+                  const float *__restrict__ bg, float *__restrict__ out_color,
+                  float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
+                  float *__restrict__ final_T) {
+    render_fwd_body<PPL, U, LAZY, false>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, 0);
+}
+
+// the batched forward: the default sub-tile shape <1,1> only (8 CTAs per SM, as render_fwd_kernel<1,1>)
+template <bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads, 8)
+render_views_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+                  const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
+                  int two_ended, int sms, CostOrder co, unsigned *__restrict__ lazy_note,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
+                  const float *__restrict__ bg, float *__restrict__ out_color,
+                  float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
+                  float *__restrict__ final_T, int tiles_view) {
+    render_fwd_body<1, 1, LAZY, true>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, tiles_view);
+}
+
 // ----------------------------------------------------------------------------------------------------------------
 // Backward.
 // ----------------------------------------------------------------------------------------------------------------
@@ -382,15 +431,17 @@ struct BwdSmem {
 // ROWSUM = the step-2 accumulation uses that the 8 pixels a lane covers per pass lie on ONE pixel row: dy is constant over them, so
 // only sum u, sum u dx, sum u dx^2 run per pixel and the three dy moments follow from them per row (5 instead of 8 floating-point
 // instructions per (record, pixel) on the u side).  ROWSUM = false keeps the per-pixel form (A/B: dgr_set_tuning bit 26).
-template <int PPL, int U, bool LAZY, bool ROWSUM = true>
-__global__ void __launch_bounds__(kRenderThreads)
-render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
+// VIEWS: the batched backward (dgr_views_backward), tiles and images numbered as in render_fwd_body; the moments go to the
+// records of the batch (the ids the sort wrote are record numbers v P + g).
+template <int PPL, int U, bool LAZY, bool ROWSUM, bool VIEWS>
+__device__ __forceinline__ void
+render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
                   unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
                   const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ lazy_note,
                   const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
                   const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
                   const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
-                  float *__restrict__ grad_rec) {
+                  float *__restrict__ grad_rec, int tiles_view) {
     using ST = SubTile<PPL>;
     using SM = BwdSmem<PPL>;
     constexpr int kPix = SM::kPix;
@@ -415,7 +466,8 @@ render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
         for (int o = 1; o < 32; o <<= 1) { const unsigned t = __shfl_up_sync(0xffffffffu, cum_end, o); if (lane >= o) cum_end += t; }
     }
     const unsigned n_items = by_cost ? __shfl_sync(0xffffffffu, cum_end, 31) : __ldcg(n_tiles_nonempty) * (unsigned)ST::kPerTile;
-    const float b0 = __ldg(bg), b1 = __ldg(bg + 1), b2 = __ldg(bg + 2);
+    float b0 = 0.f, b1 = 0.f, b2 = 0.f;
+    if (!VIEWS) { b0 = __ldg(bg); b1 = __ldg(bg + 1); b2 = __ldg(bg + 2); }
     const size_t HW = (size_t)H * W;
     const int my_r = lane & (kBatch - 1), my_q = lane / kBatch;      // step 2: parked record, pixel group
 
@@ -434,9 +486,21 @@ render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
         const unsigned ot = by_cost ? item / 8u : item / ST::kPerTile;
         const int tile = (int)__ldcg(tile_order + ot), sub = (int)(by_cost ? item % 8u : item % ST::kPerTile);
         const uint2 range = __ldcg(order_ranges + ot);
-        const int tx = tile % gx, ty = tile / gx;
+        int v = 0, lt = tile;
+        if (VIEWS) { v = tile / tiles_view; lt = tile - v * tiles_view; }
+        const int tx = lt % gx, ty = lt / gx;
         const int wx0 = ST::x0(tx, sub), wy0 = ST::y0(ty, sub);
         const int wx1 = wx0 + ST::kW - 1, wy1 = wy0 + ST::kH - 1;
+        const float *vfT = final_T, *vgC = gC, *vgD = gD, *vgA = gA;
+        const unsigned *vnc = n_contrib;
+        if (VIEWS) {
+            b0 = __ldg(bg + 3 * v); b1 = __ldg(bg + 3 * v + 1); b2 = __ldg(bg + 3 * v + 2);
+            const size_t vb = (size_t)v * HW;
+            vfT += vb; vnc += vb;
+            if (gC) vgC += 3 * vb;
+            if (gD) vgD += vb;
+            if (gA) vgA += vb;
+        }
 
         float fx[PPL], fy[PPL], gc0[PPL], gc1[PPL], gc2[PPL], gd[PPL], ga[PPL], T[PPL], R[PPL];
         unsigned last[PPL];
@@ -448,11 +512,11 @@ render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
             gc0[p] = 0.f; gc1[p] = 0.f; gc2[p] = 0.f; gd[p] = 0.f; ga[p] = 0.f; T[p] = 1.f; last[p] = 0;
             if ((x < W) && (y < H)) {
                 const size_t pix = (size_t)y * W + x;
-                last[p] = __ldcg(n_contrib + pix);
-                T[p] = __ldcg(final_T + pix);
-                if (gC) { gc0[p] = __ldg(gC + pix); gc1[p] = __ldg(gC + HW + pix); gc2[p] = __ldg(gC + 2 * HW + pix); }
-                if (gD) gd[p] = __ldg(gD + pix);
-                if (gA) ga[p] = __ldg(gA + pix);
+                last[p] = __ldcg(vnc + pix);
+                T[p] = __ldcg(vfT + pix);
+                if (gC) { gc0[p] = __ldg(vgC + pix); gc1[p] = __ldg(vgC + HW + pix); gc2[p] = __ldg(vgC + 2 * HW + pix); }
+                if (gD) gd[p] = __ldg(vgD + pix);
+                if (gA) ga[p] = __ldg(vgA + pix);
             }
             // R = T_final * (bg . gC) + sum over Gaussians behind the current one of w * s
             R[p] = T[p] * (b0 * gc0[p] + b1 * gc1[p] + b2 * gc2[p]);
@@ -637,6 +701,31 @@ render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
         if (nslots > 0) flush();
         __syncwarp();
     }
+}
+
+template <int PPL, int U, bool LAZY, bool ROWSUM = true>
+__global__ void __launch_bounds__(kRenderThreads)
+render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
+                  unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ lazy_note,
+                  const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
+                  const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
+                  const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
+                  float *__restrict__ grad_rec) {
+    render_bwd_body<PPL, U, LAZY, ROWSUM, false>(H, W, gx, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, 0);
+}
+
+// the batched backward: the default sub-tile shape <1,2> with the per-row step 2 only
+template <bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads)
+render_views_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
+                  unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ lazy_note,
+                  const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
+                  const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
+                  const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
+                  float *__restrict__ grad_rec, int tiles_view) {
+    render_bwd_body<1, 2, LAZY, true, true>(H, W, gx, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, tiles_view);
 }
 
 }  // namespace dgr

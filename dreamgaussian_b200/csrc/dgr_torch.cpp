@@ -195,6 +195,149 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
     return g;
 }
 
+// ---- batched cameras (DgrViews, dgr_views_*): one cloud, V same-size views per call ----------------------------------------
+struct ViewsState {
+    DgrViews s;
+    DgrGaussians g;
+    Tensor tanfov, bg, view, proj, campos;
+    Tensor means3D, opac;
+    OptTensor sh, scales, rots, sh_rest;
+    Tensor geom, binning, image, radii;
+    int64_t capacity = 0, n_inst = 0;
+    int32_t staging = DGR_STAGING_SORTED;
+    int device = 0;
+};
+
+std::unordered_map<uint64_t, Hint> g_views_hints;       // keyed by (device, P, H, W, V), apart from the single-view hints
+uint64_t views_hint_key(int dev, int64_t P, int H, int W, int V) {
+    uint64_t h = 1469598103934665603ull;
+    for (uint64_t x : {(uint64_t)dev, (uint64_t)P, (uint64_t)H, (uint64_t)W, (uint64_t)V}) { h ^= x; h *= 1099511628211ull; }
+    return h;
+}
+
+// instance capacity the binning buffer may be sized for: the 32-bit positions of the kernels, and half the free device memory
+int64_t views_capacity_ceiling(int64_t V, int64_t H, int64_t W) {
+    size_t free_b = 0, total_b = 0;
+    int64_t ceil = 0xfffffffell;
+    if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
+        const int64_t per = (int64_t)dgr_views_binning_bytes(1 << 20, (int32_t)V, (int32_t)H, (int32_t)W) >> 20;   // bytes per instance
+        ceil = std::min<int64_t>(ceil, std::max<int64_t>(65536, (int64_t)(free_b / 2) / std::max<int64_t>(per, 1)));
+    }
+    return ceil;
+}
+
+std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
+views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov, const Tensor &bg,
+              const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh, const Tensor &opac,
+              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+    auto st = std::make_shared<ViewsState>();
+    st->means3D = dev_f32(means3D, "means3D");
+    const c10::cuda::CUDAGuard guard(st->means3D.device());
+    st->device = st->means3D.get_device();
+    st->opac = dev_f32(opac, "opacities");
+    st->tanfov = dev_f32(tanfov, "tanfov"); st->bg = dev_f32(bg, "bg"); st->view = dev_f32(view, "viewmatrix");
+    st->proj = dev_f32(proj, "projmatrix"); st->campos = dev_f32(campos, "campos");
+    const int64_t V = st->bg.size(0);
+    TORCH_CHECK_VALUE(st->tanfov.numel() == 2 * V && st->bg.numel() == 3 * V && st->view.numel() == 16 * V && st->proj.numel() == 16 * V &&
+                      st->campos.numel() == 3 * V, "per-view tanfov [V,2], bg / campos [V,3], viewmatrix / projmatrix [V,16] expected");
+    st->sh = dev_f32(sh, "shs"); st->scales = dev_f32(scales, "scales"); st->rots = dev_f32(rots, "rotations");
+    st->sh_rest = activations ? opt_f32(sh_rest, "features_rest") : c10::nullopt;
+    if (st->sh_rest.has_value() && st->sh_rest->numel() == 0) st->sh_rest = c10::nullopt;
+    TORCH_CHECK_VALUE(st->means3D.dim() == 2 && st->means3D.size(1) == 3, "means3D must have dimensions (num_points, 3)");
+    const int64_t P = st->means3D.size(0);
+    TORCH_CHECK_VALUE(st->sh->dim() == 3 && st->sh->size(0) == P && st->sh->size(2) == 3, "shs must have dimensions (num_points, num_coeffs, 3)");
+    int64_t M = st->sh->size(1);
+    if (activations) {
+        TORCH_CHECK_VALUE(M == 1, "features_dc must have dimensions (num_points, 1, 3)");
+        if (st->sh_rest.has_value()) {
+            TORCH_CHECK_VALUE(st->sh_rest->dim() == 3 && st->sh_rest->size(0) == P && st->sh_rest->size(2) == 3, "features_rest must have dimensions (num_points, num_coeffs - 1, 3)");
+            M = 1 + st->sh_rest->size(1);
+        }
+    }
+    TORCH_CHECK_VALUE(st->scales->numel() == P * 3, "scales must have dimensions (num_points, 3)");
+    TORCH_CHECK_VALUE(st->rots->numel() == P * 4, "rotations must have dimensions (num_points, 4)");
+    TORCH_CHECK_VALUE(st->opac.numel() == P, "opacities must have dimensions (num_points, 1)");
+    st->s = DgrViews{(int32_t)V, (int32_t)H, (int32_t)W, (float)scale_modifier, (int32_t)sh_degree, debug ? 1 : 0, st->tanfov.data_ptr<float>(),
+                     st->bg.data_ptr<float>(), st->view.data_ptr<float>(), st->proj.data_ptr<float>(), st->campos.data_ptr<float>()};
+    st->g = DgrGaussians{(int32_t)P, (int32_t)M, st->means3D.numel() ? st->means3D.data_ptr<float>() : nullptr, fptr(st->sh), nullptr,
+                         st->opac.numel() ? st->opac.data_ptr<float>() : nullptr, fptr(st->scales), fptr(st->rots), nullptr,
+                         fptr(st->sh_rest), activations ? 1 : 0};
+    const auto f32 = st->means3D.options();
+    const auto u8 = f32.dtype(torch::kUInt8);
+    Tensor color = torch::empty({V, 3, H, W}, f32), depth = torch::empty({V, 1, H, W}, f32), alpha = torch::empty({V, 1, H, W}, f32);
+    st->radii = torch::empty({V, P}, f32.dtype(torch::kInt32));
+    st->geom = torch::empty({(int64_t)dgr_views_geom_bytes((int32_t)V, (int32_t)P, (int32_t)H, (int32_t)W)}, u8);
+    st->image = torch::empty({(int64_t)dgr_views_image_bytes((int32_t)V, (int32_t)H, (int32_t)W)}, u8);
+    void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
+    check(dgr_views_forward_preprocess(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), stream));
+    DgrImages out{color.data_ptr<float>(), depth.data_ptr<float>(), alpha.data_ptr<float>(), st->radii.data_ptr<int32_t>()};
+    const int64_t ceiling = views_capacity_ceiling(V, H, W);
+    Hint hint{std::min<int64_t>(std::max<int64_t>(65536, 16 * P * V), ceiling), true};
+    const uint64_t key = views_hint_key(st->device, P, (int)H, (int)W, (int)V);
+    { std::lock_guard<std::mutex> lk(g_mu); auto it = g_views_hints.find(key); if (it != g_views_hints.end()) hint = it->second; }
+    SyncObjs &so = sync_objs(st->device);
+    int64_t cap = hint.cap, n_inst = 0, n_big = 0;
+    bool big = hint.big;
+    int rerun = 0;
+    while (true) {
+        st->binning = torch::empty({(int64_t)dgr_views_binning_bytes((uint64_t)cap, (int32_t)V, (int32_t)H, (int32_t)W)}, u8);
+        const uint64_t ticket = ++so.ticket;
+        volatile uint64_t *cnt = reinterpret_cast<volatile uint64_t *>(so.counts.data_ptr<int64_t>());
+        check(dgr_views_forward_render(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
+                                       (big ? DGR_FLAG_BIG_TILES : 0) | rerun, reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>()), ticket,
+                                       nullptr, stream));
+        {
+            pybind11::gil_scoped_release nogil;
+            uint64_t spins = 0;
+            while (cnt[2] != ticket) {
+                if ((++spins & 0xfffff) == 0) {
+                    const cudaError_t q = cudaStreamQuery((cudaStream_t)stream);
+                    if (q != cudaErrorNotReady && cnt[2] != ticket) {
+                        TORCH_CHECK(q == cudaSuccess, "libdgr_b200: forward failed on the device: ", cudaGetErrorString(q));
+                        TORCH_CHECK(false, "libdgr_b200: the instance count never arrived (is the count buffer device-mapped?)");
+                    }
+                }
+            }
+        }
+        n_inst = so.counts.data_ptr<int64_t>()[0]; n_big = so.counts.data_ptr<int64_t>()[1];
+        if (n_inst <= cap && (big || n_big == 0)) break;
+        TORCH_CHECK(n_inst < 0xffffffffll, "libdgr_b200: the batch has ", n_inst, " tile instances, above the 2^32-1 the kernels address");
+        cap = std::min<int64_t>(std::max<int64_t>(cap, (int64_t)(n_inst * 1.25) + 4096), 0xfffffffell);
+        big = big || n_big > 0;
+        rerun = DGR_FLAG_RERUN;
+    }
+    { std::lock_guard<std::mutex> lk(g_mu);
+      g_views_hints[key] = Hint{std::min<int64_t>(std::max<int64_t>((int64_t)(n_inst * 1.25) + 4096, 65536), 0xfffffffell), n_big > 0}; }
+    st->capacity = cap; st->n_inst = n_inst; st->staging = (int32_t)so.counts.data_ptr<int64_t>()[3];
+    return {color, st->radii, depth, alpha, st};
+}
+
+// grads: (means3D, means2D [V,P,3], shs | features_dc, opacities, scales, rotations, features_rest); the per-Gaussian ones summed over views
+std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
+                                   bool accumulate, const std::vector<OptTensor> &out) {
+    const c10::cuda::CUDAGuard guard(st->means3D.device());
+    const int64_t P = st->g.P, M = st->g.M, V = st->s.V;
+    const auto f32 = st->means3D.options();
+    OptTensor c = gC.has_value() && gC->defined() ? OptTensor(dev_f32(*gC, "grad_color")) : c10::nullopt;
+    OptTensor d = gD.has_value() && gD->defined() ? OptTensor(dev_f32(*gD, "grad_depth")) : c10::nullopt;
+    OptTensor a = gA.has_value() && gA->defined() ? OptTensor(dev_f32(*gA, "grad_alpha")) : c10::nullopt;
+    std::vector<Tensor> g(7);
+    auto pick = [&](size_t i, bool wanted, c10::IntArrayRef shape) {
+        if (i < out.size() && out[i].has_value() && out[i]->defined()) g[i] = *out[i];
+        else if (wanted) g[i] = torch::empty(shape, f32);
+    };
+    const bool act = st->g.activations != 0;
+    pick(0, true, {P, 3}); pick(1, true, {V, P, 3}); pick(2, true, {P, act ? 1 : M, 3}); pick(3, true, {P, 1});
+    pick(4, true, {P, 3}); pick(5, true, {P, 4}); pick(6, act && st->sh_rest.has_value(), {P, M - 1, 3});
+    auto gp = [&](size_t i) -> float * { return g[i].defined() && g[i].numel() > 0 ? g[i].data_ptr<float>() : nullptr; };
+    DgrImageGrads gin{fptr(c), fptr(d), fptr(a)};
+    DgrGaussianGrads gout{gp(0), gp(1), gp(2), nullptr, gp(3), gp(4), gp(5), nullptr, accumulate ? 1 : 0, gp(6), nullptr, nullptr, nullptr, nullptr};
+    void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
+    check(dgr_views_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
+                             st->radii.data_ptr<int32_t>(), &gin, &gout, stream));
+    return g;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -205,6 +348,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("backward", &backward, "backward through the C ABI", pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"),
           pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"),
           pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0);
+    pybind11::class_<ViewsState, std::shared_ptr<ViewsState>>(m, "ViewsState")
+        .def_readonly("capacity", &ViewsState::capacity)
+        .def_readonly("num_rendered", &ViewsState::n_inst);
+    m.def("views_forward", &views_forward, "both forward stages of the batched-camera call through the C ABI");
+    m.def("views_backward", &views_backward, "backward of the batched-camera call through the C ABI", pybind11::arg("state"),
+          pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"));
+    m.def("set_views_hint", [](int dev, int64_t P, int H, int W, int V, int64_t cap, bool big) {
+        std::lock_guard<std::mutex> lk(g_mu); g_views_hints[views_hint_key(dev, P, H, W, V)] = Hint{cap, big}; });
+    m.def("get_views_hint", [](int dev, int64_t P, int H, int W, int V) -> pybind11::object {
+        std::lock_guard<std::mutex> lk(g_mu);
+        auto it = g_views_hints.find(views_hint_key(dev, P, H, W, V));
+        if (it == g_views_hints.end()) return pybind11::none();
+        return pybind11::make_tuple(it->second.cap, it->second.big); });
     m.def("abi_version", []() { return dgr_abi_version(); });
     m.def("set_hint", [](int dev, int64_t P, int H, int W, int64_t cap, bool big) {
         std::lock_guard<std::mutex> lk(g_mu); g_hints[hint_key(dev, P, H, W)] = Hint{cap, big}; });

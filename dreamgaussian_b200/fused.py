@@ -78,7 +78,7 @@ class _RasterizeRaw(torch.autograd.Function):
         d_op, d_sc, d_rot = torch.empty((P, 1), **f32), torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
         stats = ctx.stats.as_tuple() if ctx.stats is not None else None
         _r.backward_impl(state, gC, gD, gA, d_xyz, d_m2d, d_dc, None, d_op, d_sc, d_rot, None, d_sh_rest=d_rest, densify=stats)
-        return d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot, None, None
+        return d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None
 
 
 class FusedGaussianRasterizer(nn.Module):
@@ -107,3 +107,33 @@ def render_gaussian_model(gaussians, raster_settings, stats: Optional[DensifySta
         means2D=means2D, stats=stats)
     return {"image": color.clamp(0, 1), "depth": depth, "alpha": alpha, "viewspace_points": means2D,
             "visibility_filter": radii > 0, "radii": radii}
+
+
+class _RasterizeViewsRaw(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xyz, means2D, features_dc, features_rest, opacity_raw, scaling_raw, rotation_raw, settings_list):
+        xyz = _r._dev_f32(xyz, "xyz")
+        dc = _r._dev_f32(features_dc, "features_dc")
+        rest = _r._opt(features_rest, "features_rest")
+        if rest is not None and rest.numel() == 0:
+            rest = None
+        op, sc, rot = _r._dev_f32(opacity_raw, "opacity"), _r._dev_f32(scaling_raw, "scaling"), _r._dev_f32(rotation_raw, "rotation")
+        color, radii, depth, alpha, state = _r.views_forward_impl(settings_list, xyz, dc, op, sc, rot, sh_rest=rest, activations=True)
+        ctx.state = state
+        ctx.mark_non_differentiable(radii)
+        return color, radii, depth, alpha
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
+        d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot = _r._views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=True)
+        return d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None
+
+
+def rasterize_views_raw(settings_list, xyz, means2D, features_dc, features_rest, opacity, scaling, rotation):
+    """rasterize_views (rasterizer.py) for GaussianModel's RAW parameters: one cloud, a batch of same-size cameras, the
+    activations applied in the kernels and the gradients summed over the views with respect to the raw tensors.  means2D
+    [V,P,3] receives the per-view screen-space gradient.  The densification statistics are not updated by the batched call."""
+    settings_list = _r._check_views_settings(settings_list)
+    if means2D is not None and tuple(means2D.shape) != (len(settings_list), xyz.shape[0], 3):
+        raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
+    return _RasterizeViewsRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, settings_list)

@@ -344,3 +344,219 @@ class GaussianRasterizer(nn.Module):
             raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
                                    self.raster_settings)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Batched cameras: one cloud, V views of the same image size in one forward / backward (include/dgr_b200.h, DgrViews).
+# ---------------------------------------------------------------------------------------------------------------------------
+def get_views_capacity_hint(device_index, P, H, W, V):
+    """Instance-capacity hint of the batched call, kept apart from the single-view hints."""
+    if _FAST is not None:
+        return _FAST.get_views_hint(device_index, P, H, W, V)
+    return _CAPACITY_HINT.get(("views", device_index, P, H, W, V))
+
+
+def set_views_capacity_hint(device_index, P, H, W, V, cap, big):
+    if _FAST is not None:
+        _FAST.set_views_hint(device_index, P, H, W, V, cap, big)
+    else:
+        _CAPACITY_HINT[("views", device_index, P, H, W, V)] = (cap, big)
+
+
+_MAX_CAPACITY = 2 ** 32 - 2          # tile-instance positions are 32-bit in the kernels
+
+
+def _views_capacity_ceiling(lib, dev, V, H, W):
+    """Largest instance capacity a batched call sizes its binning buffer for: the kernels' 32-bit positions, and half the free
+    device memory (the first-call guess of 16 instances per record would ask for tens of GB at 64 views x 1M Gaussians)."""
+    free, _ = torch.cuda.mem_get_info(dev)
+    per = max(1, lib.dgr_views_binning_bytes(1 << 20, V, H, W) >> 20)
+    return min(_MAX_CAPACITY, max(65536, (free // 2) // per))
+
+
+def _check_views_settings(settings_list):
+    settings_list = list(settings_list)
+    if not settings_list:
+        raise ValueError("rasterize_views needs at least one camera")
+    if len(settings_list) > _lib.VIEWS_MAX:
+        raise ValueError("rasterize_views takes at most %d cameras per call, got %d" % (_lib.VIEWS_MAX, len(settings_list)))
+    s0 = settings_list[0]
+    for i, s in enumerate(settings_list[1:], 1):
+        for f in ("image_height", "image_width", "sh_degree", "scale_modifier"):
+            if getattr(s, f) != getattr(s0, f):
+                raise ValueError("rasterize_views: every camera of a batch must share %s (camera 0 has %r, camera %d has %r)"
+                                 % (f, getattr(s0, f), i, getattr(s, f)))
+    return settings_list
+
+
+def _views_cameras(settings_list, dev):
+    """The per-view device arrays of a batch: tanfov [V,2], bg [V,3], viewmatrix [V,16], projmatrix [V,16], campos [V,3]."""
+    stack = lambda name: torch.stack([_dev_f32(getattr(s, name), name).reshape(-1) for s in settings_list]).to(dev)
+    bg, view, proj, campos = stack("bg"), stack("viewmatrix"), stack("projmatrix"), stack("campos")
+    if bg.shape[1] != 3 or view.shape[1] != 16 or proj.shape[1] != 16 or campos.shape[1] != 3:
+        raise ValueError("bg/campos must have 3 elements, viewmatrix/projmatrix 16")
+    tanfov = torch.tensor([[float(s.tanfovx), float(s.tanfovy)] for s in settings_list], dtype=torch.float32, device=dev)
+    return tanfov, bg, view, proj, campos
+
+
+class _Views:
+    """ctypes views of one batched call's cameras + inputs (keeps the tensors alive)."""
+
+    def __init__(self, settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False):
+        dev = means3D.device
+        s0 = settings_list[0]
+        V = len(settings_list)
+        self.tanfov, self.bg, self.view, self.proj, self.campos = _views_cameras(settings_list, dev)
+        self.keep = [self.bg, self.view, self.proj, self.campos, self.tanfov]
+        self.V, self.H, self.W = V, int(s0.image_height), int(s0.image_width)
+        self.settings = _lib.DgrViews(V, self.H, self.W, float(s0.scale_modifier), int(s0.sh_degree), int(bool(s0.debug)),
+                                      _ptr(self.tanfov), _ptr(self.bg), _ptr(self.view), _ptr(self.proj), _ptr(self.campos))
+        # the per-Gaussian checks of the single-view call (shapes, raw-parameter layout)
+        fr = _Frame(s0, means3D, sh, None, opacities, scales, rotations, None, sh_rest, activations)
+        self.P, self.M, self.gaussians = fr.P, fr.M, fr.gaussians
+        self.keep.append(fr)
+
+
+class ViewsState:
+    """Everything one batched forward leaves behind for its backward."""
+    __slots__ = ("views", "capacity", "staging", "num_rendered", "geom", "binning", "image", "radii", "tensors", "fast")
+
+
+def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False):
+    """Both forward stages of the batched call through the C ABI; inputs are validated CUDA float32 tensors.
+    Returns (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W], ViewsState).  Same speculative-capacity
+    protocol as forward_impl, with hints keyed by (device, P, H, W, V); the compiled host layer when it is loaded."""
+    lib = _lib.load()
+    dev = means3D.device
+    if _FAST is not None:
+        s0 = settings_list[0]
+        with torch.cuda.device(dev):
+            cams = _views_cameras(settings_list, dev)
+        color, radii, depth, alpha, cst = _FAST.views_forward(
+            int(s0.image_height), int(s0.image_width), float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams,
+            means3D, sh, opacities, scales, rotations, sh_rest, bool(activations))
+        state = ViewsState()
+        state.fast, state.capacity, state.num_rendered, state.radii = cst, cst.capacity, cst.num_rendered, radii
+        state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
+        return color, radii, depth, alpha, state
+    with torch.cuda.device(dev):
+        vw = _Views(settings_list, means3D, sh, opacities, scales, rotations, sh_rest, activations)
+        V, H, W, P = vw.V, vw.H, vw.W, vw.P
+        u8 = dict(dtype=torch.uint8, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        color, depth, alpha = torch.empty((V, 3, H, W), **f32), torch.empty((V, 1, H, W), **f32), torch.empty((V, 1, H, W), **f32)
+        radii = torch.empty((V, P), dtype=torch.int32, device=dev)
+        geom = torch.empty((lib.dgr_views_geom_bytes(V, P, H, W),), **u8)
+        image = torch.empty((lib.dgr_views_image_bytes(V, H, W),), **u8)
+        n_host, event = _host_sync_objects(dev)
+        st = _stream_ptr(dev)
+        _lib.check(lib.dgr_views_forward_preprocess(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(image),
+                                                    _ptr(radii), st))
+        out = _lib.DgrImages(_ptr(color), _ptr(depth), _ptr(alpha), _ptr(radii))
+        key = ("views", dev.index, P, H, W, V)
+        ceiling = _views_capacity_ceiling(lib, dev, V, H, W)
+        cap, big = _CAPACITY_HINT.get(key, (min(max(65536, 16 * P * V), ceiling), True))
+        rerun = 0
+        while True:
+            binning = torch.empty((lib.dgr_views_binning_bytes(cap, V, H, W),), **u8)
+            _lib.check(lib.dgr_views_forward_render(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(binning),
+                                                    ctypes.c_uint64(cap), _ptr(image), ctypes.byref(out), (1 if big else 0) | rerun,
+                                                    ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event, st))
+            _lib.check(lib.dgr_event_synchronize(event))
+            n_inst, n_big = int(n_host[0]), int(n_host[1])
+            if n_inst <= cap and (big or n_big == 0):
+                break
+            if n_inst > _MAX_CAPACITY:
+                raise RuntimeError("libdgr_b200: the batch has %d tile instances, above the 2^32-1 the kernels address" % n_inst)
+            cap = min(max(cap, int(n_inst * 1.25) + 4096), _MAX_CAPACITY)
+            big = big or n_big > 0
+            rerun = 2                                   # DGR_FLAG_RERUN
+        _CAPACITY_HINT[key] = (min(max(int(n_inst * 1.25) + 4096, 65536), _MAX_CAPACITY), n_big > 0)
+    state = ViewsState()
+    state.fast = None
+    state.views, state.capacity, state.staging, state.num_rendered = vw, cap, int(n_host[3]), n_inst
+    state.geom, state.binning, state.image, state.radii = geom, binning, image, radii
+    state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
+    return color, radii, depth, alpha, state
+
+
+def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot,
+                        accumulate=False, d_sh_rest=None):
+    """Backward of a batched forward: the per-Gaussian gradients are the sums over the views (written, or added with
+    accumulate); d_means2D is per view, [V,P,3]."""
+    if state.fast is not None:
+        _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate),
+                             [d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest])
+        return
+    lib = _lib.load()
+    vw = state.views
+    dev = state.radii.device
+    with torch.cuda.device(dev):
+        gin = _lib.DgrImageGrads(_ptr(grad_color), _ptr(grad_depth), _ptr(grad_alpha))
+        gout = _lib.DgrGaussianGrads(_ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), None, _ptr(d_opac), _ptr(d_scales), _ptr(d_rot),
+                                     None, 1 if accumulate else 0, _ptr(d_sh_rest), None, None, None, None)
+        _lib.check(lib.dgr_views_backward(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning),
+                                          ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii),
+                                          ctypes.byref(gin), ctypes.byref(gout), _stream_ptr(dev)))
+
+
+def _views_grads(state, grad_color, grad_depth, grad_alpha, raw):
+    """-> (means3D, means2D [V,P,3], shs | features_dc, features_rest, opacities, scales, rotations) gradients."""
+    if state.fast is not None:
+        g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [])       # undefined -> None
+        return g[0], g[1], g[2], g[6], g[3], g[4], g[5]
+    means3D, sh, opacities, scales, rotations, sh_rest = state.tensors
+    vw = state.views
+    P, M, V = vw.P, vw.M, vw.V
+    f32 = dict(dtype=torch.float32, device=means3D.device)
+    gC = _dev_f32(grad_color, "grad_color") if grad_color is not None else None
+    gD = _dev_f32(grad_depth, "grad_depth") if grad_depth is not None else None
+    gA = _dev_f32(grad_alpha, "grad_alpha") if grad_alpha is not None else None
+    d_means3D, d_means2D, d_opac = torch.empty((P, 3), **f32), torch.empty((V, P, 3), **f32), torch.empty((P, 1), **f32)
+    d_sh = torch.empty((P, 1 if raw else M, 3), **f32)
+    d_rest = torch.empty(sh_rest.shape, **f32) if (raw and sh_rest is not None) else None
+    d_scales, d_rot = torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
+    views_backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest=d_rest)
+    return d_means3D, d_means2D, d_sh, d_rest, d_opac, d_scales, d_rot
+
+
+class _RasterizeViews(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list):
+        means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
+        sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
+        color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations)
+        ctx.state = state
+        ctx.mark_non_differentiable(radii)
+        return color, radii, depth, alpha
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
+        d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=False)
+        # ctx.state stays: a retain_graph backward runs again from the same buffers.  means2D may be None (no per-view gradient wanted)
+        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None
+
+
+def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rotations):
+    """Renders ONE cloud from every camera of `settings_list` (GaussianRasterizationSettings, at most 64, all with the same
+    image_height / image_width / sh_degree / scale_modifier) in one batched forward, and one batched backward.
+    Returns (color [V,3,H,W], radii int32 [V,P], depth [V,1,H,W], alpha [V,1,H,W]); view v equals what GaussianRasterizer
+    returns for camera v.  The gradients of means3D / shs / opacities / scales / rotations are summed over the views;
+    means2D is [V,P,3] (e.g. zeros with requires_grad) or None: its gradient is per view, for densification.  SH colours and
+    scale / rotation inputs only; no CPU path."""
+    settings_list = _check_views_settings(settings_list)
+    if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
+        raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
+    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list)
+
+
+class GaussianViewsRasterizer(nn.Module):
+    """`GaussianRasterizer` for a batch of same-size cameras: forward(means3D, means2D, opacities, shs, scales, rotations)
+    -> (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]), see rasterize_views."""
+
+    def __init__(self, settings_list):
+        super().__init__()
+        self.settings_list = _check_views_settings(settings_list)
+
+    def forward(self, means3D, means2D, opacities, shs, scales, rotations):
+        return rasterize_views(self.settings_list, means3D, means2D, opacities, shs, scales, rotations)

@@ -182,6 +182,51 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom, const 
                  uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii, const float *out_alpha,
                  const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream);
 
+/* == Batched cameras: ONE cloud rendered from V cameras of the same image size in one forward / backward ==
+ * Every view has its own camera and background; image size, SH degree and scale modifier are shared.  All arrays are DEVICE
+ * arrays.  Outputs: DgrImages.color [V,3,H,W], depth / alpha [V,1,H,W], radii [V,P] int32; view v is what dgr_forward_* returns
+ * for camera v (up to the rounding of fused multiply-adds, which ptxas chooses per kernel).  The backward SUMS the gradients of
+ * means3D / shs / opacities / scales / rotations over the views (written, or added with DgrGaussianGrads.accumulate) and writes
+ * dL_dmeans2D per view, [V,P,3].
+ * Supported inputs: SH + scale / rotation, plain or raw (DgrGaussians.activations).  Refused before any device work:
+ * colors_precomp / cov3D_precomp, the densification statistics (xyz_gradient_accum / denom / max_radii2D) and DgrPeerPush.
+ * Limits, checked before any device work: 1 <= V <= DGR_VIEWS_MAX; V x tiles per view <= 51200 (the shared-memory tile
+ * histogram of the single-view call, now spanning the batch); V x P <= DGR_VIEWS_MAX_RECORDS (record r = v P + g is the 32-bit
+ * id the sort keys carry); every image-size limit of the single-view call.
+ * Scratch: geom holds V x P records and moments (dgr_views_geom_bytes), image V x tiles per-tile arrays and [V,H,W] pixel state.
+ * Kernel shapes: the batched render kernels are the default sub-tile shapes only (forward 8x4 pixels per warp, one hit at a time;
+ * backward 8x4 with two hits together and the per-row step 2): dgr_set_tuning's pixels-per-lane, hits-together and bit 26 do not
+ * apply to them.  The scheduling knobs (cost order, two-ended queue, CTAs per SM, PDL), record staging (bits 22-23), input
+ * staging of the forward (bit 24) and the sort buckets (bit 28) do. */
+#define DGR_VIEWS_MAX 64
+#define DGR_VIEWS_MAX_RECORDS 2147483647ll
+typedef struct DgrViews {
+    int32_t V;
+    int32_t image_height;
+    int32_t image_width;
+    float   scale_modifier;
+    int32_t sh_degree;       /* active degree, 0..3 */
+    int32_t debug;           /* !=0: synchronise and check after every kernel */
+    const float *tanfov;     /* [V,2]   tanfovx, tanfovy */
+    const float *bg;         /* [V,3]   */
+    const float *viewmatrix; /* [V,4,4] row-major, as DgrSettings.viewmatrix */
+    const float *projmatrix; /* [V,4,4] */
+    const float *campos;     /* [V,3]   */
+} DgrViews;
+
+size_t dgr_views_geom_bytes(int32_t V, int32_t P, int32_t image_height, int32_t image_width);
+size_t dgr_views_image_bytes(int32_t V, int32_t image_height, int32_t image_width);
+size_t dgr_views_binning_bytes(uint64_t capacity_instances, int32_t V, int32_t image_height, int32_t image_width);
+/* As dgr_forward_preprocess / dgr_forward_render / dgr_backward, for the batch (same capacity, DGR_FLAG_BIG_TILES, ticket and
+ * counts_host[0..3] protocol; `staging` = the counts_host[3] the batched forward left).  radii: [V,P]. */
+int dgr_views_forward_preprocess(const DgrViews *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii, void *stream);
+int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geom, void *binning, uint64_t capacity_instances,
+                             void *image, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                             void *count_ready_event, void *stream);
+int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom, const void *binning, uint64_t capacity_instances,
+                       int32_t staging, const void *image, const int32_t *radii, const DgrImageGrads *gin,
+                       const DgrGaussianGrads *gout, void *stream);
+
 /* Multi-GPU (view-sharded data parallelism, SURVEY.md §8e): all-reduce(sum) of the flat float32 gradient buffer over
  * NVLink with this library's own kernel.  The buffer lives in symmetric memory: peer_ptrs[w] (HOST array of `world` device
  * addresses) is rank w's copy mapped into this process; multicast_ptr, if non-zero, is the NVSwitch multicast address of
