@@ -149,34 +149,34 @@ inline bool stage_inputs_ok(const DgrGaussians *g, bool raw) {
 }
 constexpr size_t kMaxKernelSmem = 227 * 1024;
 
+// Dynamic shared memory of a per-Gaussian forward kernel: the tile histogram, then, when its inputs are staged by bulk TMA,
+// 8 warps x 32 x (44 + 12 M) bytes from stage_off.  Staged when the kernel has a staged variant (stageable: SH + scale /
+// rotation inputs), the knob allows it, the inputs qualify and it fits next to the kernel's static shared memory.
+struct PreFwdSmem { size_t bytes, stage_off; bool staged; };
+PreFwdSmem pre_fwd_smem(const DgrGaussians *g, bool stageable, bool raw, int tiles, size_t static_smem) {
+    const size_t hist = (size_t)tiles * 4, stage_off = align_up(hist, 128);
+    const size_t staged_bytes = stage_off + (size_t)(kPreThreads / 32) * stage_warp_floats(g->M) * 4;
+    const bool staged = stageable && g_stage_fwd.load() && stage_inputs_ok(g, raw) && staged_bytes + static_smem + 1024 <= kMaxKernelSmem;
+    return { staged ? staged_bytes : hist, staged ? stage_off : 0, staged };
+}
+
+
 template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW>
 void launch_pre_fwd(const DgrSettings *s, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L, unsigned *tile_count,
                     cudaStream_t st) {
-    unsigned *run_matrix = reinterpret_cast<unsigned *>(geom + L.off_runs);
-    const size_t hist = (size_t)L.tiles * 4;
+    const PreFwdSmem sm = pre_fwd_smem(g, HAS_SH && !HAS_COV, RAW, L.tiles, 0);
+    auto launch = [&](auto kernel) {
+        if (sm.bytes > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.bytes);
+        launch_k(kernel, dim3(L.nblocks), dim3(kPreThreads), sm.bytes, st, false,
+            g->P, g->M, s->image_height, s->image_width, s->tanfovx, s->tanfovy, s->scale_modifier, s->viewmatrix, s->projmatrix,
+            s->campos, g->means3D, g->shs, g->shs_rest, g->colors_precomp, g->opacities, g->scales, g->rotations, g->cov3D_precomp, radii,
+            reinterpret_cast<Rec *>(geom + L.off_rec), reinterpret_cast<unsigned *>(geom + L.off_touched),
+            tile_count, reinterpret_cast<unsigned *>(geom + L.off_runs), L.tiles, L.iters, (int)sm.stage_off);
+    };
     if constexpr (HAS_SH && !HAS_COV) {
-        // inputs staged through shared memory by bulk TMA: [tile histogram | 8 warps x 32 x (44 + 12 M) bytes]
-        const size_t stage_off = align_up(hist, 128);
-        const size_t smem = stage_off + (size_t)(kPreThreads / 32) * stage_warp_floats(g->M) * 4;
-        if (g_stage_fwd.load() && stage_inputs_ok(g, RAW) && smem + 1024 <= kMaxKernelSmem) {
-            if (smem > 48 * 1024)
-                cudaFuncSetAttribute(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            launch_k(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>, dim3(L.nblocks), dim3(kPreThreads), smem, st, false,
-                g->P, g->M, s->image_height, s->image_width, s->tanfovx, s->tanfovy, s->scale_modifier, s->viewmatrix, s->projmatrix,
-                s->campos, g->means3D, g->shs, g->shs_rest, g->colors_precomp, g->opacities, g->scales, g->rotations, g->cov3D_precomp, radii,
-                reinterpret_cast<Rec *>(geom + L.off_rec), reinterpret_cast<unsigned *>(geom + L.off_touched),
-                tile_count, run_matrix, L.tiles, L.iters, (int)stage_off);
-            return;
-        }
+        if (sm.staged) return launch(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>);
     }
-    const size_t smem = hist;
-    if (smem > 48 * 1024)
-        cudaFuncSetAttribute(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    launch_k(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, dim3(L.nblocks), dim3(kPreThreads), smem, st, false,
-        g->P, g->M, s->image_height, s->image_width, s->tanfovx, s->tanfovy, s->scale_modifier, s->viewmatrix, s->projmatrix,
-        s->campos, g->means3D, g->shs, g->shs_rest, g->colors_precomp, g->opacities, g->scales, g->rotations, g->cov3D_precomp, radii,
-        reinterpret_cast<Rec *>(geom + L.off_rec), reinterpret_cast<unsigned *>(geom + L.off_touched),
-        tile_count, run_matrix, L.tiles, L.iters, 0);
+    launch(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>);
 }
 
 template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW>
@@ -305,6 +305,76 @@ int persistent_grid(DevInfo *d, K kernel, int threads, size_t smem) {
     d->grids[key] = g;
     return g;
 }
+
+// ---- launch steps shared by the single-view and the batched (dgr_views_*) entry points ---------------------------------------
+// A forward re-run with corrected capacity guesses repeats everything from instance emission on: the per-tile totals and run
+// matrix are still valid, what the first, clipped render pass filed as backward costs is not.
+int clear_costs_for_rerun(char *image, const ImageLayout &IL, int tiles, cudaStream_t st) {
+    DGR_CUDA(cudaMemsetAsync(image + IL.off_cost, 0, (size_t)tiles * 8 * 4, st));
+    DGR_CUDA(cudaMemsetAsync(image + IL.off_work + offsetof(TileWork, cost_bpt), 0, sizeof(TileWork) - offsetof(TileWork, cost_bpt), st));
+    return 0;
+}
+
+// Without a ticket: { n_instances, n_big_tiles } to the host and the count-ready event, between the emit kernel and the sort
+// (this also ends the chain of programmatic dependent launches there).
+int copy_counts(const char *geom, uint64_t *counts_host, uint64_t ticket, void *count_ready_event, cudaStream_t st) {
+    if (ticket) return 0;
+    if (counts_host) DGR_CUDA(cudaMemcpyAsync(counts_host, geom, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    if (count_ready_event) DGR_CUDA(cudaEventRecord((cudaEvent_t)count_ready_event, st));
+    return 0;
+}
+
+// Record staging of the render kernels.  A sorted copy of the records (written by the sort kernel, read with one contiguous
+// bulk-TMA copy per 32 records) is the fast path while that copy lives in L2; once it is several times the L2 size the
+// sort kernel's gather + write becomes the long pole and staging by id wins although a chunk then takes 32 small bulk
+// copies (tools/tma_gather_probe.cu times both).  The threshold follows the device's L2 size (50 MB on an H100).
+// Decided once per forward: its backward must stage its records the same way (the sorted copy is not written when staging
+// by id), whatever the knobs say by then — the caller hands counts_host[3] to the backward.  Returns true for staging by id.
+bool stage_records_by_id(uint64_t capacity, const DevInfo *dv, uint64_t *counts_host) {
+    const int lz = g_lazy.load();
+    const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
+    if (counts_host) counts_host[3] = lazy ? DGR_STAGING_BY_ID : DGR_STAGING_SORTED;
+    return lazy;
+}
+
+// The per-tile sorts of the instance keys (+ the record gather unless lazy): the small-tile sorter over every tile, then the
+// big-tile sorter when the emit kernel found big tiles.
+int launch_tile_sorts(DevInfo *dv, const char *image, const ImageLayout &IL, int tiles, bool big_tiles, bool lazy,
+                      unsigned long long *keys, const Rec *rec, unsigned *ids, Rec *recs, int debug, cudaStream_t st) {
+    const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
+    const uint2 *oranges = reinterpret_cast<const uint2 *>(image + IL.off_oranges);
+    if (g_sort_fine.load()) {
+        const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBucketsFine>, kSortSmallThreads, SmSF::bytes));
+        DGR_KERNEL("tile_sort_gather", st, debug,
+                   launch_k(tile_sort_gather_kernel<kSortSmallBucketsFine>, dim3(sort_grid), dim3(kSortSmallThreads), SmSF::bytes, st, true, work,
+                            oranges, keys, rec, ids, recs, lazy ? 0 : 1));
+    } else {
+        const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBuckets>, kSortSmallThreads, SmS::bytes));
+        DGR_KERNEL("tile_sort_gather", st, debug,
+                   launch_k(tile_sort_gather_kernel<kSortSmallBuckets>, dim3(sort_grid), dim3(kSortSmallThreads), SmS::bytes, st, true, work,
+                            oranges, keys, rec, ids, recs, lazy ? 0 : 1));
+    }
+    if (big_tiles)
+        DGR_KERNEL("tile_sort_gather_big", st, debug,
+                   launch_k(tile_sort_gather_big_kernel, dim3(dv->big_grid), dim3(kSortBigThreads), SmB::bytes, st, true, work,
+                            reinterpret_cast<const unsigned *>(image + IL.off_biglist), reinterpret_cast<const uint2 *>(image + IL.off_ranges),
+                            keys, rec, ids, recs, lazy ? 0 : 1));
+    return 0;
+}
+
+// Work order of the render kernels by the cost the forward measured (dgr_render.cuh), or none when that knob is off.  bwd_ppl =
+// the sub-tile shape of the backward the costs are grouped for.  (The backward only reads what the forward wrote.)
+CostOrder cost_order(const char *image, const ImageLayout &IL, int tiles, int bwd_ppl) {
+    CostOrder co{};
+    if (g_cost_order.load()) {
+        char *im = const_cast<char *>(image);
+        TileWork *work = reinterpret_cast<TileWork *>(im + IL.off_work);
+        co.cost_acc = reinterpret_cast<unsigned *>(im + IL.off_cost); co.cls_count = work->cls_count;
+        co.cls_items = reinterpret_cast<unsigned *>(im + IL.off_clsitems); co.cost_bpt = &work->cost_bpt;
+        co.tiles = tiles; co.bwd_ppl = bwd_ppl;
+    }
+    return co;
+}
 }  // namespace
 
 extern "C" {
@@ -418,13 +488,8 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v
     TileWork *work = reinterpret_cast<TileWork *>(image + IL.off_work);
     DevInfo *dv = dev_info();
     if (!dv) return -1;
-    (void)(flags & DGR_FLAG_RERUN);           // a re-run only repeats the scan from the (still valid) per-tile totals
-    // (a re-run with corrected guesses repeats everything from here: per-tile totals and run matrix are still valid; what the
-    //  first, clipped render pass filed as backward costs is not)
-    if (flags & DGR_FLAG_RERUN) {
-        DGR_CUDA(cudaMemsetAsync(image + IL.off_cost, 0, (size_t)tiles * 8 * 4, st));
-        DGR_CUDA(cudaMemsetAsync(reinterpret_cast<char *>(work) + offsetof(TileWork, cost_bpt), 0, sizeof(TileWork) - offsetof(TileWork, cost_bpt), st));
-    }
+    if (flags & DGR_FLAG_RERUN)
+        if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
     {
         // instance emission; its extra block publishes ranges / order / counts (capacity 0: only that block has work to do)
         const size_t smem = (size_t)tiles * 4;
@@ -435,45 +500,13 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v
                             run_matrix, keys, ranges, hdr, tile_order, reinterpret_cast<uint2 *>(image + IL.off_oranges), work, big_list,
                             (volatile unsigned long long *)(ticket ? counts_host : nullptr), (unsigned long long)ticket));
     }
-    if (!ticket) {            // copy + event between the kernels (this also ends the chain of programmatic dependent launches here)
-        if (counts_host)      // { n_instances, n_big_tiles }
-            DGR_CUDA(cudaMemcpyAsync(counts_host, geom, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        if (count_ready_event) DGR_CUDA(cudaEventRecord((cudaEvent_t)count_ready_event, st));
-    }
-    // Record staging of the render kernels.  A sorted copy of the records (written by the sort kernel, read with one contiguous
-    // bulk-TMA copy per 32 records) is the fast path while that copy lives in L2; once it is several times the L2 size the
-    // sort kernel's gather + write becomes the long pole and staging by id wins although a chunk then takes 32 small bulk
-    // copies (tools/tma_gather_probe.cu times both).  The threshold follows the device's L2 size (50 MB on an H100).
-    // Decided here once: the backward of this call must stage its records the same way (the sorted copy is not written when
-    // staging by id), whatever the knobs say by then — the caller hands counts_host[3] to dgr_backward.
-    const int lz = g_lazy.load();
-    const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
-    if (counts_host) counts_host[3] = lazy ? DGR_STAGING_BY_ID : DGR_STAGING_SORTED;
-    if (g->P > 0 && capacity > 0) {
-        if (g_sort_fine.load()) {
-            const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBucketsFine>, kSortSmallThreads, SmSF::bytes));
-            DGR_KERNEL("tile_sort_gather", st, s->debug,
-                       launch_k(tile_sort_gather_kernel<kSortSmallBucketsFine>, dim3(sort_grid), dim3(kSortSmallThreads), SmSF::bytes, st, true, (const TileWork *)work,
-                                reinterpret_cast<const uint2 *>(image + IL.off_oranges), keys, rec, ids, recs, lazy ? 0 : 1));
-        } else {
-            const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBuckets>, kSortSmallThreads, SmS::bytes));
-            DGR_KERNEL("tile_sort_gather", st, s->debug,
-                       launch_k(tile_sort_gather_kernel<kSortSmallBuckets>, dim3(sort_grid), dim3(kSortSmallThreads), SmS::bytes, st, true, (const TileWork *)work,
-                                reinterpret_cast<const uint2 *>(image + IL.off_oranges), keys, rec, ids, recs, lazy ? 0 : 1));
-        }
-        if (flags & DGR_FLAG_BIG_TILES)
-            DGR_KERNEL("tile_sort_gather_big", st, s->debug,
-                       launch_k(tile_sort_gather_big_kernel, dim3(dv->big_grid), dim3(kSortBigThreads), SmB::bytes, st, true, (const TileWork *)work,
-                                (const unsigned *)big_list, (const uint2 *)ranges, keys, rec, ids, recs, lazy ? 0 : 1));
-    }
+    if (int e = copy_counts(geom, counts_host, ticket, count_ready_event, st)) return e;
+    const bool lazy = stage_records_by_id(capacity, dv, counts_host);
+    if (g->P > 0 && capacity > 0)
+        if (int e = launch_tile_sorts(dv, image, IL, tiles, flags & DGR_FLAG_BIG_TILES, lazy, keys, rec, ids, recs, s->debug, st)) return e;
     // persistent forward render: every (tile, sub-tile) is a work item, handed out heaviest tile first
     const int ppl = g_ppl_fwd.load(), uf = g_u_fwd.load();
-    CostOrder co{};
-    if (g_cost_order.load()) {
-        co.cost_acc = reinterpret_cast<unsigned *>(image + IL.off_cost); co.cls_count = work->cls_count;
-        co.cls_items = reinterpret_cast<unsigned *>(image + IL.off_clsitems); co.cost_bpt = &work->cost_bpt;
-        co.tiles = tiles; co.bwd_ppl = g_ppl_bwd.load();
-    }
+    const CostOrder co = cost_order(image, IL, tiles, g_ppl_bwd.load());
 #define DGR_RENDER_FWD_L(PPL_, U_, L_)                                                                          \
     do {                                                                                                        \
         const int items_ = tiles * SubTile<PPL_>::kPerTile;                                                     \
@@ -544,13 +577,7 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
         const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
         unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
         const int ppl = g_ppl_bwd.load(), ub = g_u_bwd.load();
-        CostOrder co{};
-        if (g_cost_order.load()) {            // (read-only here; the kernel checks that the forward grouped its costs for this shape)
-            TileWork *wk = const_cast<TileWork *>(work);
-            co.cost_acc = const_cast<unsigned *>(reinterpret_cast<const unsigned *>(image + IL.off_cost)); co.cls_count = wk->cls_count;
-            co.cls_items = const_cast<unsigned *>(reinterpret_cast<const unsigned *>(image + IL.off_clsitems)); co.cost_bpt = &wk->cost_bpt;
-            co.tiles = tiles; co.bwd_ppl = ppl == 1 ? 1 : 2;
-        }
+        const CostOrder co = cost_order(image, IL, tiles, ppl == 1 ? 1 : 2);     // (the kernel checks that the forward grouped its costs for this shape)
 #define DGR_RENDER_BWD_L(PPL_, U_, L_)                                                                                        \
     do {                                                                                                                   \
         const size_t smem_ = sizeof(BwdSmem<PPL_>) * kRenderWarps;                                                         \
@@ -633,24 +660,17 @@ constexpr size_t kViewsFwdStaticSmem = (size_t)kMaxViews * (sizeof(FrameConsts) 
 template <int DEG, bool RAW>
 void launch_views_pre_fwd(const DgrViews *s, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L, int tiles_view,
                           unsigned *tile_count, cudaStream_t st) {
-    unsigned *run_matrix = reinterpret_cast<unsigned *>(geom + L.off_runs);
-    const size_t hist = (size_t)L.tiles * 4;
-    // staged path: [tile histogram of the batch | 8 warps x 32 x (44 + 12 M) bytes], when it fits next to the cameras
-    const size_t stage_off = align_up(hist, 128);
-    const size_t smem_st = stage_off + (size_t)(kPreThreads / 32) * stage_warp_floats(g->M) * 4;
-    const bool staged = g_stage_fwd.load() && stage_inputs_ok(g, RAW) && smem_st + kViewsFwdStaticSmem + 1024 <= kMaxKernelSmem;
-    const size_t smem = staged ? smem_st : hist;
-#define DGR_VIEWS_PRE_FWD(STG_)                                                                                                   \
-    do {                                                                                                                         \
-        if (smem + kViewsFwdStaticSmem > 48 * 1024)          /* the cameras' static shared memory counts against the 48 KB */    \
-            cudaFuncSetAttribute(preprocess_views_fwd_kernel<DEG, RAW, STG_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        launch_k(preprocess_views_fwd_kernel<DEG, RAW, STG_>, dim3(L.nblocks), dim3(kPreThreads), smem, st, false, g->P, g->M, s->V,   \
-                 s->image_height, s->image_width, s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos, g->means3D,   \
-                 g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, radii, reinterpret_cast<Rec *>(geom + L.off_rec),          \
-                 reinterpret_cast<unsigned *>(geom + L.off_touched), tile_count, run_matrix, tiles_view, L.iters, (int)stage_off);     \
-    } while (0)
-    if (staged) DGR_VIEWS_PRE_FWD(true); else DGR_VIEWS_PRE_FWD(false);
-#undef DGR_VIEWS_PRE_FWD
+    const PreFwdSmem sm = pre_fwd_smem(g, true, RAW, L.tiles, kViewsFwdStaticSmem);
+    auto launch = [&](auto kernel) {
+        if (sm.bytes + kViewsFwdStaticSmem > 48 * 1024)          // the cameras' static shared memory counts against the 48 KB
+            cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.bytes);
+        launch_k(kernel, dim3(L.nblocks), dim3(kPreThreads), sm.bytes, st, false, g->P, g->M, s->V, s->image_height, s->image_width,
+                 s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos, g->means3D, g->shs, g->shs_rest, g->opacities,
+                 g->scales, g->rotations, radii, reinterpret_cast<Rec *>(geom + L.off_rec), reinterpret_cast<unsigned *>(geom + L.off_touched),
+                 tile_count, reinterpret_cast<unsigned *>(geom + L.off_runs), tiles_view, L.iters, (int)sm.stage_off);
+    };
+    if (sm.staged) launch(preprocess_views_fwd_kernel<DEG, RAW, true>);
+    else launch(preprocess_views_fwd_kernel<DEG, RAW, false>);
 }
 
 template <int DEG, bool RAW>
@@ -734,10 +754,8 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
     TileWork *work = reinterpret_cast<TileWork *>(image + IL.off_work);
     DevInfo *dv = dev_info();
     if (!dv) return -1;
-    if (flags & DGR_FLAG_RERUN) {
-        DGR_CUDA(cudaMemsetAsync(image + IL.off_cost, 0, (size_t)tiles * 8 * 4, st));
-        DGR_CUDA(cudaMemsetAsync(reinterpret_cast<char *>(work) + offsetof(TileWork, cost_bpt), 0, sizeof(TileWork) - offsetof(TileWork, cost_bpt), st));
-    }
+    if (flags & DGR_FLAG_RERUN)
+        if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
     {
         const int nb = (g->P > 0 && capacity > 0) ? GL.nblocks : 0;
         DGR_KERNEL("emit_views", st, s->debug,
@@ -746,37 +764,11 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
                             (unsigned long long)capacity, run_matrix, keys, ranges, hdr, tile_order, reinterpret_cast<uint2 *>(image + IL.off_oranges),
                             work, big_list, (volatile unsigned long long *)(ticket ? counts_host : nullptr), (unsigned long long)ticket));
     }
-    if (!ticket) {
-        if (counts_host) DGR_CUDA(cudaMemcpyAsync(counts_host, geom, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        if (count_ready_event) DGR_CUDA(cudaEventRecord((cudaEvent_t)count_ready_event, st));
-    }
-    // record staging: the rule of dgr_forward_render, reported to the caller for the backward
-    const int lz = g_lazy.load();
-    const bool lazy = lz == 2 || (lz == 0 && (size_t)capacity * sizeof(Rec) > 2 * dv->l2_bytes);
-    if (counts_host) counts_host[3] = lazy ? DGR_STAGING_BY_ID : DGR_STAGING_SORTED;
-    if (g->P > 0 && capacity > 0) {
-        if (g_sort_fine.load()) {
-            const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBucketsFine>, kSortSmallThreads, SmSF::bytes));
-            DGR_KERNEL("tile_sort_gather", st, s->debug,
-                       launch_k(tile_sort_gather_kernel<kSortSmallBucketsFine>, dim3(sort_grid), dim3(kSortSmallThreads), SmSF::bytes, st, true, (const TileWork *)work,
-                                reinterpret_cast<const uint2 *>(image + IL.off_oranges), keys, rec, ids, recs, lazy ? 0 : 1));
-        } else {
-            const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBuckets>, kSortSmallThreads, SmS::bytes));
-            DGR_KERNEL("tile_sort_gather", st, s->debug,
-                       launch_k(tile_sort_gather_kernel<kSortSmallBuckets>, dim3(sort_grid), dim3(kSortSmallThreads), SmS::bytes, st, true, (const TileWork *)work,
-                                reinterpret_cast<const uint2 *>(image + IL.off_oranges), keys, rec, ids, recs, lazy ? 0 : 1));
-        }
-        if (flags & DGR_FLAG_BIG_TILES)
-            DGR_KERNEL("tile_sort_gather_big", st, s->debug,
-                       launch_k(tile_sort_gather_big_kernel, dim3(dv->big_grid), dim3(kSortBigThreads), SmB::bytes, st, true, (const TileWork *)work,
-                                (const unsigned *)big_list, (const uint2 *)ranges, keys, rec, ids, recs, lazy ? 0 : 1));
-    }
-    CostOrder co{};
-    if (g_cost_order.load()) {
-        co.cost_acc = reinterpret_cast<unsigned *>(image + IL.off_cost); co.cls_count = work->cls_count;
-        co.cls_items = reinterpret_cast<unsigned *>(image + IL.off_clsitems); co.cost_bpt = &work->cost_bpt;
-        co.tiles = tiles; co.bwd_ppl = 1;                       // the batched backward's 8x4 sub-tiles
-    }
+    if (int e = copy_counts(geom, counts_host, ticket, count_ready_event, st)) return e;
+    const bool lazy = stage_records_by_id(capacity, dv, counts_host);
+    if (g->P > 0 && capacity > 0)
+        if (int e = launch_tile_sorts(dv, image, IL, tiles, flags & DGR_FLAG_BIG_TILES, lazy, keys, rec, ids, recs, s->debug, st)) return e;
+    const CostOrder co = cost_order(image, IL, tiles, 1);          // the batched backward's 8x4 sub-tiles
 #define DGR_VIEWS_FWD(L_)                                                                                                   \
     do {                                                                                                                   \
         const int items_ = tiles * SubTile<1>::kPerTile;                                                                   \
@@ -824,13 +816,7 @@ int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, c
         if (!dv) return -1;
         const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
         unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
-        CostOrder co{};
-        if (g_cost_order.load()) {
-            TileWork *wk = const_cast<TileWork *>(work);
-            co.cost_acc = const_cast<unsigned *>(reinterpret_cast<const unsigned *>(image + IL.off_cost)); co.cls_count = wk->cls_count;
-            co.cls_items = const_cast<unsigned *>(reinterpret_cast<const unsigned *>(image + IL.off_clsitems)); co.cost_bpt = &wk->cost_bpt;
-            co.tiles = tiles; co.bwd_ppl = 1;
-        }
+        const CostOrder co = cost_order(image, IL, tiles, 1);
         const bool lazy = staging == DGR_STAGING_BY_ID;
 #define DGR_VIEWS_BWD(L_)                                                                                                       \
     do {                                                                                                                       \

@@ -588,13 +588,10 @@ preprocess_views_bwd_kernel(int P, int M, int V, int H, int W, float scale_modif
     }
     // the SH row is re-read per view (L1) instead of being held in registers next to the gradient sums
     const float *shrow = RAW ? shs_rest + (size_t)g * (M - 1) * 3 : shs + (size_t)g * M * 3;
-    float R[9], S6[6], inv_qnorm = 1.f;
-    float3 s = s_in;
-    if (RAW) s = make_float3(expf(s.x), expf(s.y), expf(s.z));
-    s = make_float3(scale_modifier * s.x, scale_modifier * s.y, scale_modifier * s.z);
-    float4 q = q_in;
-    if (RAW) q = act_normalize(q, inv_qnorm);
-    quat_to_R(q, R);
+    float R[9], S6[6], inv_qnorm;
+    float3 s;
+    float4 q;
+    activate_scale_rot<RAW>(s_in, q_in, scale_modifier, s, q, inv_qnorm, R);
     cov3d_from_scale_rot(s, R, S6);
     const float o = RAW ? act_sigmoid(o_in) : o_in;
 

@@ -282,68 +282,16 @@ emit_instances_kernel(int P, int gx, int tiles, int gpb_iters, int nblocks, cons
         tile_meta_cta<kPreThreads>(tiles, tile_count, cap, ranges, hdr, tile_order, order_ranges, work, big_list, counts_host, ticket);
         return;
     }
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // range starts: exclusive scan of the per-tile totals.  Warp w owns the contiguous tile range [w R, (w + 1) R); its lanes
-    // read 32 consecutive tiles at a time (coalesced, several loads in flight): pass 1 sums the range, pass 2 (after the
-    // warp bases are known) scans it and adds the block's run-matrix row.
-    constexpr int NW = kPreThreads / 32;
-    const int R = ((tiles + NW - 1) / NW + 31) / 32 * 32;
-    const int w_lo = min(tiles, warp * R), w_hi = min(tiles, w_lo + R);
-    unsigned long long sum = 0;
-#pragma unroll 4
-    for (int t = w_lo + lane; t < w_hi; t += 32) sum += __ldcg(tile_count + t);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if (lane == 0) s_part[warp] = sum;
-    __syncthreads();
-    unsigned long long run = 0;
-    for (int w = 0; w < warp; w++) run += s_part[w];
-    const unsigned *row = run_matrix + (size_t)blockIdx.x * tiles;
-    // (the totals and run-matrix entries of kE 32-tile pieces are requested before the first of them is scanned: the scans form
-    //  a dependent chain through `run`, and one L2 round trip per piece would otherwise sit in front of every link of it)
-    constexpr int kE = 4;
-    for (int t0 = w_lo; t0 < w_hi; t0 += 32 * kE) {
-        unsigned cj[kE], rj[kE];
-#pragma unroll
-        for (int j = 0; j < kE; j++) {
-            const int t = t0 + 32 * j + lane;
-            cj[j] = t < w_hi ? __ldcg(tile_count + t) : 0u;
-            rj[j] = t < w_hi ? __ldcg(row + t) : 0u;
-        }
-#pragma unroll
-        for (int j = 0; j < kE; j++) {
-            if (t0 + 32 * j < w_hi) {                                     // warp-uniform
-                const int t = t0 + 32 * j + lane;
-                const unsigned c = cj[j];
-                unsigned inc = c;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) { const unsigned n = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += n; }
-                const unsigned long long start = run + (inc - c);
-                if (t < w_hi) s_off[t] = (unsigned)(start < cap ? start : cap) + rj[j];
-                run += __shfl_sync(0xffffffffu, inc, 31);
-            }
-        }
-    }
-    __syncthreads();
+    emit_block_cursors(tiles, tile_count, cap, run_matrix, s_off, s_part);
     const unsigned cap32 = (unsigned)cap;
     for (int it = 0; it < gpb_iters; it++) {
-        const int g = (int)((blockIdx.x * gpb_iters + it) * kPreThreads + tid);
+        const int g = (int)((blockIdx.x * gpb_iters + it) * kPreThreads + threadIdx.x);
         if (g >= P) continue;
         const int cnt = (int)(__ldg(touched + g) & 0x1fffffffu);                  // = tw * th (same AABB as the histogram)
         if (cnt == 0) continue;
         const float4 q1 = __ldg(&rec[g].q1);
         const unsigned long long key = ((unsigned long long)__float_as_uint(q1.z) << 32) | (unsigned)g;
-        const unsigned ax = __float_as_uint(q1.w), ay = __float_as_uint(__ldg(&rec[g].q2.w));
-        const int tx0 = (int)(ax & 0xffffu) >> 4, tw = ((int)(ax >> 16) >> 4) - tx0 + 1;
-        const int ty0 = (int)(ay & 0xffffu) >> 4;
-        int x = 0, t = ty0 * gx + tx0;
-#pragma unroll 4
-        for (int i = 0; i < cnt; i++) {
-            const unsigned pos = atomicAdd(&s_off[t], 1u);
-            if (pos < cap32) keys[pos] = key;                             // beyond the instance capacity: dropped
-            x++; t++;
-            if (x == tw) { x = 0; t += gx - tw; }
-        }
+        emit_keys(key, __float_as_uint(q1.w), __float_as_uint(__ldg(&rec[g].q2.w)), gx, 0, cnt, s_off, keys, cap32);
     }
 }
 

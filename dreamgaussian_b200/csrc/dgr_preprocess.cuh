@@ -262,13 +262,25 @@ __device__ __forceinline__ void ldg_gaussian(int g, int M, const float *__restri
     }
 }
 
-// Sigma from (scale, rotation) inputs (raw parameters: activations first); does not depend on the camera.
+// The scale (activated, times scale_modifier), rotation and R the forward uses for (scale, rotation) inputs; raw parameters:
+// exp and normalize first, inv_qnorm = 1 / |_rotation| (else 1).
 template <bool RAW>
-__device__ __forceinline__ void cov3d_from_inputs(float3 s, float4 q, float scale_modifier, float (&S6)[6]) {
+__device__ __forceinline__ void activate_scale_rot(float3 s_in, float4 q_in, float scale_modifier, float3 &s, float4 &q, float &inv_qnorm,
+                                                   float (&R)[9]) {
+    s = s_in;
     if (RAW) s = make_float3(expf(s.x), expf(s.y), expf(s.z));
     s = make_float3(scale_modifier * s.x, scale_modifier * s.y, scale_modifier * s.z);
-    if (RAW) { float inv; q = act_normalize(q, inv); }
-    float R[9]; quat_to_R(q, R);
+    q = q_in;
+    inv_qnorm = 1.f;
+    if (RAW) q = act_normalize(q, inv_qnorm);
+    quat_to_R(q, R);
+}
+
+// Sigma from (scale, rotation) inputs (raw parameters: activations first); does not depend on the camera.
+template <bool RAW>
+__device__ __forceinline__ void cov3d_from_inputs(float3 s_in, float4 q_in, float scale_modifier, float (&S6)[6]) {
+    float3 s; float4 q; float inv, R[9];
+    activate_scale_rot<RAW>(s_in, q_in, scale_modifier, s, q, inv, R);
     cov3d_from_scale_rot(s, R, S6);
 }
 
