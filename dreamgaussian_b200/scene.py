@@ -88,6 +88,10 @@ def make_cloud(num_pts: int, sh_degree: int = 3, seed: int = 0, radius: float = 
                opacity: str = "trained", anisotropic: bool = True, sigma: Optional[float] = None) -> dict:
     """Gaussian cloud as the op's float32 inputs: means3D, scales, rotations, opacities [P,1], shs [P,M,3].
 
+    It models a cloud at initialisation or early in training.  Saturated opacities, clamped and over-bright colours,
+    needle Gaussians, opacities at or below 1/255, sub-pixel Gaussians and Gaussians at the near plane or the frustum edge
+    (what a trained model is full of) come from the builders in tests/trained_scenes.py.
+
     opacity: "init" -> 0.1 everywhere (reference init); "trained" -> U(0.05, 0.95).
     anisotropic: per-axis sigma * exp(N(0, 0.3^2)) and random unit quaternions (else isotropic, identity).
     sigma: override the 3-NN derived isotropic scale (used by tests to avoid the kd-tree).
