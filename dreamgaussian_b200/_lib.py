@@ -83,6 +83,8 @@ EXPORTS = (
     "dgr_profile_enable", "dgr_profile_collect", "dgr_event_create", "dgr_event_synchronize", "dgr_event_destroy", "dgr_set_tuning", "dgr_peer_allreduce", "dgr_peer_flag_bytes", "dgr_peer_reduce_staged", "dgr_peer_push_flat", "dgr_knn_scratch_bytes", "dgr_dist_cuda2", "dgr_fields_scratch_bytes", "dgr_extract_fields", "dgr_adam_step", "dgr_densify_scratch_bytes", "dgr_densify_plan", "dgr_densify_apply",
     "dgr_views_geom_bytes", "dgr_views_image_bytes", "dgr_views_binning_bytes", "dgr_views_forward_preprocess",
     "dgr_views_forward_render", "dgr_views_backward",
+    "dgr_views_mixed_geom_bytes", "dgr_views_mixed_image_bytes", "dgr_views_mixed_forward_preprocess",
+    "dgr_views_mixed_forward_render", "dgr_views_mixed_backward",
 )
 
 _lib = None
@@ -178,6 +180,19 @@ def load():
     lib.dgr_views_backward.restype = ctypes.c_int
     lib.dgr_views_backward.argtypes = [ctypes.POINTER(DgrViews), ctypes.POINTER(DgrGaussians), vp, vp, u64, i32, vp, vp,
                                        ctypes.POINTER(DgrImageGrads), ctypes.POINTER(DgrGaussianGrads), vp]
+    hw = ctypes.POINTER(ctypes.c_int32)          # image_hw: host [V,2] (height, width)
+    lib.dgr_views_mixed_geom_bytes.restype = ctypes.c_size_t
+    lib.dgr_views_mixed_geom_bytes.argtypes = [i32, i32, hw]
+    lib.dgr_views_mixed_image_bytes.restype = ctypes.c_size_t
+    lib.dgr_views_mixed_image_bytes.argtypes = [i32, hw]
+    lib.dgr_views_mixed_forward_preprocess.restype = ctypes.c_int
+    lib.dgr_views_mixed_forward_preprocess.argtypes = [ctypes.POINTER(DgrViews), hw, ctypes.POINTER(DgrGaussians), vp, vp, vp, vp]
+    lib.dgr_views_mixed_forward_render.restype = ctypes.c_int
+    lib.dgr_views_mixed_forward_render.argtypes = [ctypes.POINTER(DgrViews), hw, ctypes.POINTER(DgrGaussians), vp, vp, u64, vp,
+                                                   ctypes.POINTER(DgrImages), i32, vp, u64, vp, vp]
+    lib.dgr_views_mixed_backward.restype = ctypes.c_int
+    lib.dgr_views_mixed_backward.argtypes = [ctypes.POINTER(DgrViews), hw, ctypes.POINTER(DgrGaussians), vp, vp, u64, i32, vp, vp,
+                                             ctypes.POINTER(DgrImageGrads), ctypes.POINTER(DgrGaussianGrads), u64, vp]
     if lib.dgr_abi_version() != ABI_VERSION:
         raise RuntimeError("libdgr_b200.so ABI version mismatch")
     _lib = lib

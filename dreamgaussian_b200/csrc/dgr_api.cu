@@ -623,8 +623,9 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// Batched cameras (include/dgr_b200.h, DgrViews): one cloud, V same-size views.  Same pipeline as the single-view call on a
-// global tile space (tile v T + local tile) and V x P records (record v P + g).
+// Batched cameras (include/dgr_b200.h, DgrViews): one cloud, V views, same-size (dgr_views_*) or each with its own image size
+// (dgr_views_mixed_*).  Same pipeline as the single-view call on a global tile space (view v's tiles start at tile_off[v]) and
+// V x P records (record v P + g).  Both entry families run the same five kernels; a same-size batch is the uniform ViewTable.
 // ---------------------------------------------------------------------------------------------------------------------------
 namespace {
 int check_views(const DgrViews *s) {
@@ -635,6 +636,28 @@ int check_views(const DgrViews *s) {
     if (s->sh_degree < 0 || s->sh_degree > 3) return fail(-1, "sh_degree must be 0..3");
     const size_t tiles = (size_t)((s->image_width + kTile - 1) / kTile) * (size_t)((s->image_height + kTile - 1) / kTile) * (size_t)s->V;
     if (tiles * 4 > kMaxTileSmem) return fail(-3, "views: V x tiles per view above 51200 (16x16 tiles) not supported");
+    if (!s->tanfov || !s->bg || !s->viewmatrix || !s->projmatrix || !s->campos)
+        return fail(-1, "views: tanfov / bg / viewmatrix / projmatrix / campos must not be NULL");
+    return 0;
+}
+// the mixed-size call: image_hw [V,2] (height, width) replaces DgrViews.image_height / image_width
+int check_views_mixed_sizes(const DgrViews *s, const int32_t *image_hw) {
+    if (!s) return fail(-1, "views settings is NULL");
+    if (s->V < 1 || s->V > DGR_VIEWS_MAX) return fail(-3, "views: V must be 1..64");
+    if (!image_hw) return fail(-1, "views mixed: image_hw is NULL");
+    size_t tiles = 0;
+    for (int v = 0; v < s->V; v++) {
+        const int h = image_hw[2 * v], w = image_hw[2 * v + 1];
+        if (h <= 0 || w <= 0) return fail(-1, "views mixed: every image size must be positive");
+        if (h > 65535 || w > 65535) return fail(-1, "views mixed: image size above 65535 not supported");
+        tiles += (size_t)((w + kTile - 1) / kTile) * (size_t)((h + kTile - 1) / kTile);
+    }
+    if (tiles * 4 > kMaxTileSmem) return fail(-3, "views mixed: more than 51200 tiles (16x16) in the batch not supported");
+    return 0;
+}
+int check_views_mixed(const DgrViews *s, const int32_t *image_hw) {
+    if (int e = check_views_mixed_sizes(s, image_hw)) return e;
+    if (s->sh_degree < 0 || s->sh_degree > 3) return fail(-1, "sh_degree must be 0..3");
     if (!s->tanfov || !s->bg || !s->viewmatrix || !s->projmatrix || !s->campos)
         return fail(-1, "views: tanfov / bg / viewmatrix / projmatrix / campos must not be NULL");
     return 0;
@@ -654,32 +677,68 @@ int check_views_gaussians(const DgrViews *s, const DgrGaussians *g) {
     if (g->M > 16) return fail(-1, "shs with more than 16 coefficients per channel not supported");
     return 0;
 }
+// the backward's output checks shared by both entry families (the same-size call refuses the statistics before this)
+int check_views_grads(const DgrGaussianGrads *gout) {
+    if (gout->push) return fail(-2, "views: DgrPeerPush is not supported by the batched call");
+    if (gout->dL_dcolors_precomp || gout->dL_dcov3D_precomp)
+        return fail(-2, "views: precomputed colours / cov3D are not supported by the batched call (SH + scale / rotation only)");
+    return 0;
+}
+
+// The views' sizes as the kernels see them (ViewTable) and the batch totals.  hw = V (height, width) pairs, or ONE pair for every
+// view (hw_stride 0: the same-size call).  The sizes have been checked.
+struct ViewsBatch {
+    ViewTable vt;
+    int V, tiles;
+    size_t pixels;
+};
+ViewsBatch views_batch(int V, const int32_t *hw, int hw_stride) {
+    ViewsBatch b;
+    memset(&b, 0, sizeof(b));
+    b.V = V;
+    int tiles = 0, pix = 0;
+    for (int v = 0; v < V; v++) {
+        const int h = hw[v * hw_stride], w = hw[v * hw_stride + 1];
+        b.vt.H[v] = h; b.vt.W[v] = w; b.vt.gx[v] = (w + kTile - 1) / kTile;
+        b.vt.tile_off[v] = tiles; b.vt.pix_off[v] = pix;
+        tiles += b.vt.gx[v] * ((h + kTile - 1) / kTile);
+        pix += h * w;                                   // <= 51200 tiles x 256 pixels: fits
+    }
+    for (int v = V; v <= kMaxViews; v++) b.vt.tile_off[v] = tiles;
+    b.tiles = tiles; b.pixels = (size_t)pix;
+    return b;
+}
+ViewsBatch views_batch_uniform(const DgrViews *s) {
+    const int32_t hw[2] = { s->image_height, s->image_width };
+    return views_batch(s->V, hw, 0);
+}
 
 constexpr size_t kViewsFwdStaticSmem = (size_t)kMaxViews * (sizeof(FrameConsts) + sizeof(float2)) + (kPreThreads / 32) * 8;
 
 template <int DEG, bool RAW>
-void launch_views_pre_fwd(const DgrViews *s, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L, int tiles_view,
+void launch_views_pre_fwd(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L,
                           unsigned *tile_count, cudaStream_t st) {
     const PreFwdSmem sm = pre_fwd_smem(g, true, RAW, L.tiles, kViewsFwdStaticSmem);
     auto launch = [&](auto kernel) {
         if (sm.bytes + kViewsFwdStaticSmem > 48 * 1024)          // the cameras' static shared memory counts against the 48 KB
             cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.bytes);
-        launch_k(kernel, dim3(L.nblocks), dim3(kPreThreads), sm.bytes, st, false, g->P, g->M, s->V, s->image_height, s->image_width,
+        launch_k(kernel, dim3(L.nblocks), dim3(kPreThreads), sm.bytes, st, false, g->P, g->M, s->V, b.vt,
                  s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos, g->means3D, g->shs, g->shs_rest, g->opacities,
                  g->scales, g->rotations, radii, reinterpret_cast<Rec *>(geom + L.off_rec), reinterpret_cast<unsigned *>(geom + L.off_touched),
-                 tile_count, reinterpret_cast<unsigned *>(geom + L.off_runs), tiles_view, L.iters, (int)sm.stage_off);
+                 tile_count, reinterpret_cast<unsigned *>(geom + L.off_runs), L.iters, (int)sm.stage_off);
     };
     if (sm.staged) launch(preprocess_views_fwd_kernel<DEG, RAW, true>);
     else launch(preprocess_views_fwd_kernel<DEG, RAW, false>);
 }
 
 template <int DEG, bool RAW>
-void launch_views_pre_bwd(const DgrViews *s, const DgrGaussians *g, const int *radii, const unsigned *touched, const float *grad_rec,
-                          const DgrGaussianGrads *o, cudaStream_t st) {
+void launch_views_pre_bwd(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, const int *radii, const unsigned *touched,
+                          const float *grad_rec, const DgrGaussianGrads *o, uint64_t stats_views, cudaStream_t st) {
     launch_k(preprocess_views_bwd_kernel<DEG, RAW>, dim3((g->P + kPreThreads - 1) / kPreThreads), dim3(kPreThreads), 0, st, true,
-             g->P, g->M, s->V, s->image_height, s->image_width, s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos,
+             g->P, g->M, s->V, b.vt, s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos,
              g->means3D, g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, radii, touched, grad_rec, o->dL_dmeans3D,
-             o->dL_dmeans2D, o->dL_dshs, o->dL_dopacities, o->dL_dscales, o->dL_drotations, o->dL_dshs_rest, o->accumulate);
+             o->dL_dmeans2D, o->dL_dshs, o->dL_dopacities, o->dL_dscales, o->dL_drotations, o->dL_dshs_rest, o->xyz_gradient_accum,
+             o->denom, o->max_radii2D, (unsigned long long)stats_views, o->accumulate);
 }
 
 #define DGR_VIEWS_DISPATCH(FN, ...)                                                                        \
@@ -697,50 +756,35 @@ void launch_views_pre_bwd(const DgrViews *s, const DgrGaussians *g, const int *r
             default: FN<3, false>(__VA_ARGS__); break;                                                     \
         }                                                                                                  \
     } while (0)
-}  // namespace
 
-extern "C" {
-
-size_t dgr_views_geom_bytes(int32_t V, int32_t P, int32_t H, int32_t W) { return GeomLayout(P, H, W, V > 0 ? V : 1).total; }
-size_t dgr_views_image_bytes(int32_t V, int32_t H, int32_t W) { return ImageLayout(H, W, V > 0 ? V : 1).total; }
-size_t dgr_views_binning_bytes(uint64_t cap, int32_t V, int32_t H, int32_t W) { (void)V; (void)H; (void)W; return BinningLayout(cap).total; }
-
-int dgr_views_forward_preprocess(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
-    NvtxRange nvtx_("dgr_views_forward_preprocess");
-    if (int e = check_views(s)) return e;
-    if (int e = check_views_gaussians(s, g)) return e;
+// The three stages of a checked batch (s, g and the sizes in b).
+int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
     char *geom = (char *)geom_v, *image = (char *)image_v;
     if (!geom || !image) return fail(-1, "geom / image scratch is NULL");
     if (g->P > 0 && !radii) return fail(-1, "radii is NULL");
     cudaStream_t st = (cudaStream_t)stream;
-    const int H = s->image_height, W = s->image_width;
-    GeomLayout L(g->P, H, W, s->V);
-    ImageLayout IL(H, W, s->V);
-    const int tiles_view = IL.gx * IL.gy;
+    const GeomLayout L = GeomLayout::batch(g->P, b.tiles, s->V);
+    const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
     DGR_CUDA(cudaMemsetAsync(image + IL.off_work, 0, (IL.off_cost - IL.off_work) + (size_t)L.tiles * 8 * 4, st));
     if (g->P > 0)
         DGR_KERNEL("preprocess_views_fwd", st, s->debug,
-                   DGR_VIEWS_DISPATCH(launch_views_pre_fwd, s, g, radii, geom, L, tiles_view, reinterpret_cast<unsigned *>(image + IL.off_count), st));
+                   DGR_VIEWS_DISPATCH(launch_views_pre_fwd, s, b, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), st));
     return 0;
 }
 
-int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
-                             void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
-                             void *count_ready_event, void *stream) {
-    NvtxRange nvtx_("dgr_views_forward_render");
-    if (int e = check_views(s)) return e;
-    if (int e = check_views_gaussians(s, g)) return e;
+int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                 void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket, void *count_ready_event,
+                 void *stream) {
     if (!geom_v || !image_v || !out) return fail(-1, "NULL argument");
     if (!out->color || !out->depth || !out->alpha) return fail(-1, "output images must not be NULL");
     if (capacity > 0 && !binning_v) return fail(-1, "binning scratch is NULL");
     if (capacity >= 0xffffffffull) return fail(-3, "capacity above 2^32-1 tile instances not supported");
     cudaStream_t st = (cudaStream_t)stream;
     char *geom = (char *)geom_v, *binning = (char *)binning_v, *image = (char *)image_v;
-    const int H = s->image_height, W = s->image_width;
-    GeomLayout GL(g->P, H, W, s->V);
-    ImageLayout IL(H, W, s->V);
+    const GeomLayout GL = GeomLayout::batch(g->P, b.tiles, s->V);
+    const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
     BinningLayout BL(capacity);
-    const int tiles_view = IL.gx * IL.gy, tiles = tiles_view * s->V;
+    const int tiles = b.tiles;
     uint2 *ranges = reinterpret_cast<uint2 *>(image + IL.off_ranges);
     unsigned *tile_count = reinterpret_cast<unsigned *>(image + IL.off_count);
     const unsigned *run_matrix = reinterpret_cast<const unsigned *>(geom + GL.off_runs);
@@ -759,8 +803,8 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
     {
         const int nb = (g->P > 0 && capacity > 0) ? GL.nblocks : 0;
         DGR_KERNEL("emit_views", st, s->debug,
-                   launch_k(emit_views_kernel, dim3(nb + 1), dim3(kPreThreads), (size_t)tiles * 4, st, !(flags & DGR_FLAG_RERUN), g->P, s->V, IL.gx,
-                            tiles_view, GL.iters, nb, rec, reinterpret_cast<const unsigned *>(geom + GL.off_touched), (const unsigned *)tile_count,
+                   launch_k(emit_views_kernel, dim3(nb + 1), dim3(kPreThreads), (size_t)tiles * 4, st, !(flags & DGR_FLAG_RERUN), g->P, s->V, b.vt,
+                            GL.iters, nb, rec, reinterpret_cast<const unsigned *>(geom + GL.off_touched), (const unsigned *)tile_count,
                             (unsigned long long)capacity, run_matrix, keys, ranges, hdr, tile_order, reinterpret_cast<uint2 *>(image + IL.off_oranges),
                             work, big_list, (volatile unsigned long long *)(ticket ? counts_host : nullptr), (unsigned long long)ticket));
     }
@@ -775,40 +819,29 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
         int grid_ = min(persistent_grid(dv, render_views_fwd_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
         if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                                          \
         DGR_KERNEL("render_views_fwd", st, s->debug,                                                                       \
-                   launch_k(render_views_fwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, H, W, IL.gx, \
+                   launch_k(render_views_fwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, b.vt,         \
                             (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),          \
                             (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
                             &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids, s->bg, out->color, out->depth, out->alpha, \
-                            reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT), tiles_view)); \
+                            reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT))); \
     } while (0)
     if (lazy) DGR_VIEWS_FWD(true); else DGR_VIEWS_FWD(false);
 #undef DGR_VIEWS_FWD
     return 0;
 }
 
-int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
-                       const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
-    NvtxRange nvtx_("dgr_views_backward");
-    if (int e = check_views(s)) return e;
-    if (int e = check_views_gaussians(s, g)) return e;
-    if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
-    if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
-        return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
-    if (gout->xyz_gradient_accum || gout->denom || gout->max_radii2D)
-        return fail(-2, "views: the fused densification statistics are not supported by the batched call");
-    if (gout->push) return fail(-2, "views: DgrPeerPush is not supported by the batched call");
-    if (gout->dL_dcolors_precomp || gout->dL_dcov3D_precomp)
-        return fail(-2, "views: precomputed colours / cov3D are not supported by the batched call (SH + scale / rotation only)");
+int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
+                   int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views,
+                   void *stream) {
     if (g->P == 0) return 0;
     if (!radii) return fail(-1, "radii is NULL");
     cudaStream_t st = (cudaStream_t)stream;
     char *geom = (char *)geom_v;
     const char *binning = (const char *)binning_v, *image = (const char *)image_v;
-    const int H = s->image_height, W = s->image_width;
-    GeomLayout GL(g->P, H, W, s->V);
-    ImageLayout IL(H, W, s->V);
+    const GeomLayout GL = GeomLayout::batch(g->P, b.tiles, s->V);
+    const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
     BinningLayout BL(capacity);
-    const int tiles_view = IL.gx * IL.gy, tiles = tiles_view * s->V;
+    const int tiles = b.tiles;
     float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
     DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * s->V * kGradRecFloats * 4, st));
     if (binning && capacity > 0) {
@@ -825,21 +858,113 @@ int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, c
                         (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);                                     \
         if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);                                              \
         DGR_KERNEL("render_views_bwd", st, s->debug,                                                                           \
-                   launch_k(render_views_bwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, H, W, IL.gx, \
+                   launch_k(render_views_bwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, b.vt,    \
                             reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co, \
                             reinterpret_cast<const uint2 *>(image + IL.off_oranges),                                           \
                             reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec), \
                             (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),             \
                             s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),                                     \
                             reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, \
-                            grad_rec, tiles_view));                                                                            \
+                            grad_rec));                                                                                        \
     } while (0)
         if (lazy) DGR_VIEWS_BWD(true); else DGR_VIEWS_BWD(false);
 #undef DGR_VIEWS_BWD
     }
     DGR_KERNEL("preprocess_views_bwd", st, s->debug,
-               DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, st));
+               DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, b, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout,
+                                  stats_views, st));
     return 0;
+}
+}  // namespace
+
+extern "C" {
+
+size_t dgr_views_geom_bytes(int32_t V, int32_t P, int32_t H, int32_t W) { return GeomLayout(P, H, W, V > 0 ? V : 1).total; }
+size_t dgr_views_image_bytes(int32_t V, int32_t H, int32_t W) { return ImageLayout(H, W, V > 0 ? V : 1).total; }
+size_t dgr_views_binning_bytes(uint64_t cap, int32_t V, int32_t H, int32_t W) { (void)V; (void)H; (void)W; return BinningLayout(cap).total; }
+
+int dgr_views_forward_preprocess(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
+    NvtxRange nvtx_("dgr_views_forward_preprocess");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_preprocess(s, views_batch_uniform(s), g, geom_v, image_v, radii, stream);
+}
+
+int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                             void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                             void *count_ready_event, void *stream) {
+    NvtxRange nvtx_("dgr_views_forward_render");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_render(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket,
+                        count_ready_event, stream);
+}
+
+int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                       const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
+    NvtxRange nvtx_("dgr_views_backward");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
+    if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
+        return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
+    if (gout->xyz_gradient_accum || gout->denom || gout->max_radii2D)
+        return fail(-2, "views: the fused densification statistics are not supported by the batched call");
+    if (int e = check_views_grads(gout)) return e;
+    return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, stream);
+}
+
+// ---- views of different sizes: image_hw = [V,2] (height, width) on the host ------------------------------------------------------
+size_t dgr_views_mixed_geom_bytes(int32_t V, int32_t P, const int32_t *image_hw) {
+    DgrViews s{};
+    s.V = V;
+    if (check_views_mixed_sizes(&s, image_hw)) return 0;
+    return GeomLayout::batch(P, views_batch(V, image_hw, 2).tiles, V).total;
+}
+size_t dgr_views_mixed_image_bytes(int32_t V, const int32_t *image_hw) {
+    DgrViews s{};
+    s.V = V;
+    if (check_views_mixed_sizes(&s, image_hw)) return 0;
+    const ViewsBatch b = views_batch(V, image_hw, 2);
+    return ImageLayout::batch((size_t)b.tiles, b.pixels).total;
+}
+
+int dgr_views_mixed_forward_preprocess(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, void *image_v,
+                                       int32_t *radii, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_forward_preprocess");
+    if (int e = check_views_mixed(s, image_hw)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_preprocess(s, views_batch(s->V, image_hw, 2), g, geom_v, image_v, radii, stream);
+}
+
+int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, void *binning_v,
+                                   uint64_t capacity, void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host,
+                                   uint64_t ticket, void *count_ready_event, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_forward_render");
+    if (int e = check_views_mixed(s, image_hw)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_render(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket,
+                        count_ready_event, stream);
+}
+
+int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
+                             uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                             const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_backward");
+    if (int e = check_views_mixed(s, image_hw)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
+    if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
+        return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
+    if (s->V < 64 && (stats_views >> s->V) != 0) return fail(-1, "views mixed: stats_views has a bit at or above V");
+    const bool any_stat = gout->xyz_gradient_accum || gout->denom || gout->max_radii2D;
+    if (stats_views && !any_stat)
+        return fail(-1, "views mixed: stats_views is non-zero but no densification statistic buffer is set");
+    if (!stats_views && any_stat)
+        return fail(-1, "views mixed: a densification statistic buffer is set but stats_views is 0");
+    if (int e = check_views_grads(gout)) return e;
+    return views_backward(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout,
+                          stats_views, stream);
 }
 
 }  // extern "C"

@@ -556,18 +556,22 @@ preprocess_bwd_kernel(int P, int M, int H, int W, float tanfovx, float tanfovy, 
 // Batched backward (dgr_views_backward): a thread reads its Gaussian's inputs ONCE, then applies every view's chain rule to that
 // view's moments (record v P + g) and sums in registers; the sums are written (or added) once.  The scale / rotation and opacity
 // gradients are linear in d Sigma and d L / d opacity, so only those two are summed over the views and the rest of their chain
-// rule runs once.  means2D is per view: [V, P, 3].  SH + scale / rotation inputs only (plain or raw parameters).
+// rule runs once.  means2D is per view: [V, P, 3].  SH + scale / rotation inputs only (plain or raw parameters).  View v's chain
+// rule uses its own image size (ViewTable).  Densification statistics: for every view whose bit is set in stats_views, in
+// ascending view order, a Gaussian that view rendered gets the single-view rule of preprocess_bwd_kernel with that view's means2D
+// gradient and radius (exactly what one single-view backward per selected view, in view order, leaves behind).
 // ----------------------------------------------------------------------------------------------------------------
 template <int DEG, bool RAW>
 __global__ void __launch_bounds__(kPreThreads, 3)
-preprocess_views_bwd_kernel(int P, int M, int V, int H, int W, float scale_modifier, const float *__restrict__ tanfov,
+preprocess_views_bwd_kernel(int P, int M, int V, const __grid_constant__ ViewTable vt, float scale_modifier, const float *__restrict__ tanfov,
                             const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix, const float *__restrict__ campos,
                             const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ shs_rest,
                             const float *__restrict__ opacities, const float *__restrict__ scales, const float *__restrict__ rotations,
                             const int *__restrict__ radii, const unsigned *__restrict__ touched, const float *__restrict__ grad_rec,
                             float *__restrict__ dL_dmeans3D, float *__restrict__ dL_dmeans2D, float *__restrict__ dL_dshs,
                             float *__restrict__ dL_dopacities, float *__restrict__ dL_dscales, float *__restrict__ dL_drotations,
-                            float *__restrict__ dL_dshs_rest, int accumulate) {
+                            float *__restrict__ dL_dshs_rest, float *__restrict__ xyz_gradient_accum, float *__restrict__ denom,
+                            float *__restrict__ max_radii2D, unsigned long long stats_views, int accumulate) {
     __shared__ FrameConsts s_fc[kMaxViews];
     __shared__ float2 s_tan[kMaxViews];
     __shared__ __align__(16) float s_stage[(kPreThreads / 32) * kStageFloats];
@@ -604,10 +608,11 @@ preprocess_views_bwd_kernel(int P, int M, int V, int H, int W, float scale_modif
     for (int v = 0; v < V && g < P; v++) {
         const size_t rid = (size_t)v * P + g;
         float gndx = 0.f, gndy = 0.f;
-        if (radii[rid] > 0) {
+        const int radius_v = radii[rid];
+        if (radius_v > 0) {
             const float2 tf = s_tan[v];
             float dmean[3], g_op, g_rgb[3], dS[9], bs[16], gr[3];
-            backward_camera<DEG, true, RAW>(s_fc[v], H, W, tf.x, tf.y, p, S6, o, __ldg(touched + rid) >> 29,
+            backward_camera<DEG, true, RAW>(s_fc[v], vt.H[v], vt.W[v], tf.x, tf.y, p, S6, o, __ldg(touched + rid) >> 29,
                 [&](float4 &m0, float4 &m1, float4 &m2) {
                     m0 = ldg_f4(grad_rec + rid * kGradRecFloats);
                     m1 = ldg_f4(grad_rec + rid * kGradRecFloats + 4);
@@ -623,6 +628,11 @@ preprocess_views_bwd_kernel(int P, int M, int V, int H, int W, float scale_modif
             for (int k = 0; k < NB; k++)
 #pragma unroll
                 for (int ch = 0; ch < 3; ch++) sum_sh[3 * k + ch] = __fmaf_rn(bs[k], gr[ch], sum_sh[3 * k + ch]);
+            if ((stats_views >> v) & 1ull) {
+                if (xyz_gradient_accum) xyz_gradient_accum[g] += sqrtf(gndx * gndx + gndy * gndy);
+                if (denom) denom[g] += 1.f;
+                if (max_radii2D) max_radii2D[g] = fmaxf(max_radii2D[g], (float)radius_v);
+            }
         }
         if (dL_dmeans2D) {
             float *m2d = dL_dmeans2D + rid * 3;

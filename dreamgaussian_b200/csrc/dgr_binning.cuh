@@ -296,10 +296,10 @@ emit_instances_kernel(int P, int gx, int tiles, int gpb_iters, int nblocks, cons
 }
 
 // Batched emission (dgr_views_*): the same block <-> Gaussian mapping as preprocess_views_fwd_kernel; each Gaussian appends the
-// instances of all its views: key = depth bits << 32 | record r = v P + g, in the tiles v T + local tile.  The metadata block
-// covers the V T tiles of the batch.
+// instances of all its views: key = depth bits << 32 | record r = v P + g, in the tiles tile_off[v] + local tile (ViewTable).  The
+// metadata block covers all tiles of the batch.
 __global__ void __launch_bounds__(kPreThreads)
-emit_views_kernel(int P, int V, int gx, int tiles_view, int gpb_iters, int nblocks, const Rec *__restrict__ rec, const unsigned *__restrict__ touched,
+emit_views_kernel(int P, int V, const __grid_constant__ ViewTable vt, int gpb_iters, int nblocks, const Rec *__restrict__ rec, const unsigned *__restrict__ touched,
                   const unsigned *__restrict__ tile_count, unsigned long long cap, const unsigned *__restrict__ run_matrix,
                   unsigned long long *__restrict__ keys, uint2 *__restrict__ ranges, GeomHeader *__restrict__ hdr,
                   unsigned *__restrict__ tile_order, uint2 *__restrict__ order_ranges, TileWork *__restrict__ work,
@@ -308,7 +308,7 @@ emit_views_kernel(int P, int V, int gx, int tiles_view, int gpb_iters, int nbloc
     __shared__ unsigned long long s_part[kPreThreads / 32];
     pdl_trigger();
     pdl_wait();
-    const int tiles = V * tiles_view;
+    const int tiles = vt.tile_off[V];
     if ((int)blockIdx.x == nblocks) {
         tile_meta_cta<kPreThreads>(tiles, tile_count, cap, ranges, hdr, tile_order, order_ranges, work, big_list, counts_host, ticket);
         return;
@@ -324,7 +324,7 @@ emit_views_kernel(int P, int V, int gx, int tiles_view, int gpb_iters, int nbloc
             if (cnt == 0) continue;
             const float4 q1 = __ldg(&rec[r].q1);
             const unsigned long long key = ((unsigned long long)__float_as_uint(q1.z) << 32) | r;
-            emit_keys(key, __float_as_uint(q1.w), __float_as_uint(__ldg(&rec[r].q2.w)), gx, v * tiles_view, cnt, s_off, keys, cap32);
+            emit_keys(key, __float_as_uint(q1.w), __float_as_uint(__ldg(&rec[r].q2.w)), vt.gx[v], vt.tile_off[v], cnt, s_off, keys, cap32);
         }
     }
 }

@@ -65,15 +65,22 @@ __host__ __device__ inline int choose_gpb_iters(int P, int tiles) {
 //               (the backward zeroes counter + moments with ONE memset)
 // A batch of V views of one cloud (dgr_views_*) keeps V x P records (record r = v P + g) and V x tiles-per-view tiles
 // (global tile v T + local tile); the blocks still cover the P Gaussians, so the run matrix is blocks x V T.
+// Views of different sizes (dgr_views_mixed_*): the tiles are the batch's total, sum over v of tiles_v (GeomLayout::batch).
 struct GeomLayout {
     size_t off_rec, off_touched, off_bwdwork, off_gradrec, off_runs, total;
     int tiles, iters, nblocks;
     __host__ __device__ GeomLayout(int P, int H, int W, int V = 1) {
+        int t = ((W + kTile - 1) / kTile) * ((H + kTile - 1) / kTile);
+        if (t < 1) t = 1;
+        init(P, t * V, V);
+    }
+    __host__ __device__ static GeomLayout batch(int P, int tiles_total, int V) { GeomLayout L; L.init(P, tiles_total, V); return L; }
+  private:
+    __host__ __device__ GeomLayout() {}
+    __host__ __device__ void init(int P, int tiles_total, int V) {
         size_t Pn = P > 0 ? (size_t)P : 1;
         const size_t Rn = Pn * (size_t)V;
-        tiles = ((W + kTile - 1) / kTile) * ((H + kTile - 1) / kTile);
-        if (tiles < 1) tiles = 1;
-        tiles *= V;
+        tiles = tiles_total;
         iters = choose_gpb_iters(P, tiles);
         nblocks = (int)((Pn + (size_t)kPreThreads * iters - 1) / ((size_t)kPreThreads * iters));
         size_t o = 256;
@@ -93,6 +100,8 @@ constexpr int kCostClasses = 32;         // log-scale classes of the measured fo
 //                ... [cost accumulators u32 x 8 tiles] ... [cost-class item lists u32 x 32 x 8 tiles]
 // (work, tile_count and the cost accumulators are adjacent: the forward zeroes them with ONE memset before the preprocess kernel)
 // V views (dgr_views_*): every per-tile array covers V x tiles-per-view tiles and n_contrib / final_T are [V, H, W].
+// Views of different sizes (ImageLayout::batch): the per-tile arrays cover the batch's total tiles and the pixel state its total
+// pixels, view v's [H_v, W_v] block after those of views 0 .. v-1 (gx, gy are then 0).
 struct ImageLayout {
     size_t off_ranges, off_oranges, off_count, off_cost, off_order, off_biglist, off_work, off_ncontrib, off_finalT, off_clsitems, total;
     int gx, gy;
@@ -100,7 +109,14 @@ struct ImageLayout {
         gx = (W + kTile - 1) / kTile; gy = (H + kTile - 1) / kTile;
         size_t tiles = (size_t)gx * gy; if (tiles < 1) tiles = 1;
         size_t hw = (size_t)H * W; if (hw < 1) hw = 1;
-        tiles *= (size_t)V; hw *= (size_t)V;
+        init(tiles * (size_t)V, hw * (size_t)V);
+    }
+    __host__ __device__ static ImageLayout batch(size_t tiles_total, size_t pixels_total) {
+        ImageLayout L; L.gx = 0; L.gy = 0; L.init(tiles_total, pixels_total); return L;
+    }
+  private:
+    __host__ __device__ ImageLayout() {}
+    __host__ __device__ void init(size_t tiles, size_t hw) {
         size_t o = 0;
         off_work = o;     o = align_up(o + 256, 256);
         off_count = o;    o = align_up(o + tiles * 4, 256);
@@ -115,6 +131,27 @@ struct ImageLayout {
         total = o;
     }
 };
+
+// Image sizes of the views of a batch (dgr_views_*, dgr_views_mixed_*), handed to the five batched kernels BY VALUE as a kernel
+// parameter (1.3 KB, read through the constant bank; no upload).  View v has H[v] x W[v] pixels and gx[v] tile columns; its tiles
+// are the global tiles tile_off[v] .. tile_off[v + 1] - 1 (row-major within the view) and its pixel state / images start at
+// pixel pix_off[v] (colour: float 3 pix_off[v], then [3, H_v, W_v]).  tile_off[V .. kMaxViews] = the batch's total tiles, so
+// view_of_tile needs no bound.  Same-size batches are the uniform table: tile_off[v] = v T, pix_off[v] = v H W.
+constexpr int kMaxViews = 64;
+struct ViewTable {
+    int tile_off[kMaxViews + 1];
+    int pix_off[kMaxViews];
+    int H[kMaxViews], W[kMaxViews], gx[kMaxViews];
+};
+
+// the view a global tile belongs to: binary search over tile_off (6 steps for 64 views)
+__device__ __forceinline__ int view_of_tile(const ViewTable &vt, int tile) {
+    int v = 0;
+#pragma unroll
+    for (int s = kMaxViews / 2; s > 0; s >>= 1)
+        if (vt.tile_off[v + s] <= tile) v += s;
+    return v;
+}
 
 // ------------------------------------------------ PTX wrappers ------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }

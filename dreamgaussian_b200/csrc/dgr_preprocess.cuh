@@ -569,12 +569,11 @@ preprocess_fwd_kernel(int P, int M, int H, int W, float tanfovx, float tanfovy, 
 }
 
 // ----------------------------------------------------------------------------------------------------------------
-// Batched forward (dgr_views_forward_preprocess): ONE cloud, V cameras of the same image size.  A thread reads its Gaussian's
-// inputs once (bulk-TMA staging or per-thread loads, as above) and then runs the camera-dependent part for every camera; the
-// cameras sit in shared memory.  Record r = v P + g, global tile v T + local tile (T = tiles per view); the block's histogram
-// spans all V T tiles and its run-matrix row is published once.
+// Batched forward (dgr_views_forward_preprocess, dgr_views_mixed_forward_preprocess): ONE cloud, V cameras, each with its own
+// image size (ViewTable).  A thread reads its Gaussian's inputs once (bulk-TMA staging or per-thread loads, as above) and then runs
+// the camera-dependent part for every camera; the cameras sit in shared memory.  Record r = v P + g, global tile tile_off[v] +
+// local tile; the block's histogram spans all tiles of the batch and its run-matrix row is published once.
 // ----------------------------------------------------------------------------------------------------------------
-constexpr int kMaxViews = 64;
 
 __device__ __forceinline__ void load_frames(FrameConsts *fcs, float2 *tan, int V, const float *__restrict__ tanfov,
                                             const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix,
@@ -592,18 +591,18 @@ __device__ __forceinline__ void load_frames(FrameConsts *fcs, float2 *tan, int V
 
 template <int DEG, bool RAW, bool STAGE>
 __global__ void __launch_bounds__(kPreThreads, 3)
-preprocess_views_fwd_kernel(int P, int M, int V, int H, int W, float scale_modifier, const float *__restrict__ tanfov,
+preprocess_views_fwd_kernel(int P, int M, int V, const __grid_constant__ ViewTable vt, float scale_modifier, const float *__restrict__ tanfov,
                             const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix, const float *__restrict__ campos,
                             const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ shs_rest,
                             const float *__restrict__ opacities, const float *__restrict__ scales, const float *__restrict__ rotations,
                             int *__restrict__ radii, Rec *__restrict__ rec, unsigned *__restrict__ touched_out,
-                            unsigned *__restrict__ tile_count, unsigned *__restrict__ run_matrix, int tiles_view, int gpb_iters, int stage_off) {
-    extern __shared__ __align__(128) unsigned s_hist[];                 // [V T] tile histogram | STAGE: 8 warp staging areas
+                            unsigned *__restrict__ tile_count, unsigned *__restrict__ run_matrix, int gpb_iters, int stage_off) {
+    extern __shared__ __align__(128) unsigned s_hist[];                 // [tiles of the batch] histogram | STAGE: 8 warp staging areas
     __shared__ FrameConsts s_fc[kMaxViews];
     __shared__ float2 s_tan[kMaxViews];
     __shared__ uint64_t s_stage_bar[kPreThreads / 32];
     pdl_trigger();
-    const int lane = threadIdx.x & 31, tiles = V * tiles_view, gx = (W + kTile - 1) / kTile;
+    const int lane = threadIdx.x & 31, tiles = vt.tile_off[V];
     float *wstage = STAGE ? reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(s_hist) + stage_off) + (threadIdx.x >> 5) * stage_warp_floats(M)
                           : nullptr;
     uint64_t *wbar = &s_stage_bar[threadIdx.x >> 5];
@@ -652,10 +651,10 @@ preprocess_views_fwd_kernel(int P, int M, int V, int H, int W, float scale_modif
             const float tzc = p.x * fc.V[2] + p.y * fc.V[6] + p.z * fc.V[10] + fc.V[14];
             if (tzc > DGR_NEAR_CULL_Z) {
                 const float2 tf = s_tan[v];
-                if (project_gaussian<DEG, true, RAW>(fc, H, W, tf.x, tf.y, p, S6, o_in, shc, dc0, dc1, dc2, 0.f, 0.f, 0.f, r, radius_out,
-                                                     clamp_flags)) {
-                    unsigned *vh = s_hist + v * tiles_view;
-                    for_each_touched_tile(__float_as_uint(r.q1.w), __float_as_uint(r.q2.w), gx, [&](int t) { atomicAdd(&vh[t], 1u); touched++; });
+                if (project_gaussian<DEG, true, RAW>(fc, vt.H[v], vt.W[v], tf.x, tf.y, p, S6, o_in, shc, dc0, dc1, dc2, 0.f, 0.f, 0.f, r,
+                                                     radius_out, clamp_flags)) {
+                    unsigned *vh = s_hist + vt.tile_off[v];
+                    for_each_touched_tile(__float_as_uint(r.q1.w), __float_as_uint(r.q2.w), vt.gx[v], [&](int t) { atomicAdd(&vh[t], 1u); touched++; });
                 }
             }
             const size_t rid = (size_t)v * P + g;

@@ -167,8 +167,9 @@ struct CostOrder {                       // image scratch pieces (all may be NUL
 // One-pixel-per-lane variants are held to 64 registers (8 CTAs per SM): measured 4-5 us per step at 100k / 800^2 against the
 // 72 registers ptxas picks on its own (A/B in profiles/r2_ab_variants.log).
 //
-// VIEWS: a batch of V same-size views (dgr_views_forward_render).  Tiles are numbered v T + local tile (T = tiles_view), every
-// view has its own background (bg [V,3]) and its own slices of the [V, ...] images; the records are those of the batch.
+// VIEWS: a batch of V views (dgr_views_forward_render, dgr_views_mixed_forward_render), each with its own image size (ViewTable
+// vt; H, W, gx unused).  A work item's global tile gives its view (view_of_tile: once per item) and local tile; every view has its
+// own background (bg [V,3]) and its own blocks of the flat images at pix_off[v]; the records are those of the batch.
 template <int PPL, int U, bool LAZY, bool VIEWS>
 __device__ __forceinline__ void
 render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
@@ -177,7 +178,7 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                   const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
                   const float *__restrict__ bg, float *__restrict__ out_color,
                   float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
-                  float *__restrict__ final_T, int tiles_view) {
+                  float *__restrict__ final_T, const ViewTable *vt) {
     using ST = SubTile<PPL>;
     __shared__ WarpRing rings[kRenderWarps];
     const int lane = threadIdx.x & 31;
@@ -222,8 +223,9 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
         const unsigned ot = item / ST::kPerTile;
         const int tile = (int)__ldcg(tile_order + ot), sub = (int)(item % ST::kPerTile);
         const uint2 range = __ldcg(order_ranges + ot);
-        const int v = VIEWS ? tile / tiles_view : 0, lt = VIEWS ? tile - v * tiles_view : tile;
-        const int tx = lt % gx, ty = lt / gx;
+        int v = 0, lt = tile, iW = W, iH = H, igx = gx;          // VIEWS: the item's view and its size
+        if constexpr (VIEWS) { v = view_of_tile(*vt, tile); lt = tile - vt->tile_off[v]; iW = vt->W[v]; iH = vt->H[v]; igx = vt->gx[v]; }
+        const int tx = lt % igx, ty = lt / igx;
         const int n = (int)(range.y - range.x);
         const int nchunks = (n + kChunk - 1) / kChunk;
         const Rec *src = rec_sorted + range.x;
@@ -251,7 +253,7 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
 #pragma unroll
         for (int p = 0; p < PPL; p++) {
             const int x = ST::px(wx0, lane, p), y = ST::py(wy0, lane, p);
-            inside[p] = (x < W) && (y < H);
+            inside[p] = (x < iW) && (y < iH);
             fx[p] = (float)x; fy[p] = (float)y;
             T[p] = 1.f; C0[p] = 0.f; C1[p] = 0.f; C2[p] = 0.f; D[p] = 0.f; last[p] = 0; done[p] = !inside[p];
             all_done = all_done && done[p];
@@ -325,18 +327,18 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
         // never move on (or leave) with a bulk copy in flight into this warp's ring
         for (int c = rs.waited; c < rs.issued; c++) ring_wait(rg, rs, c);
 
-        if constexpr (VIEWS) {              // view v's background and slices of the [V, ...] images
+        if constexpr (VIEWS) {              // view v's background and its [3, H_v, W_v] / [H_v, W_v] blocks at pixel pix_off[v]
             const float vb0 = __ldg(bg + 3 * v), vb1 = __ldg(bg + 3 * v + 1), vb2 = __ldg(bg + 3 * v + 2);
-            const size_t vb = (size_t)v * HW;
+            const size_t vb = (size_t)vt->pix_off[v], vhw = (size_t)iH * iW;
             float *oc = out_color + 3 * vb, *od = out_depth + vb, *oa = out_alpha + vb, *fT = final_T + vb;
             unsigned *nc = n_contrib + vb;
 #pragma unroll
             for (int p = 0; p < PPL; p++) {
                 if (inside[p]) {
-                    const size_t pix = (size_t)ST::py(wy0, lane, p) * W + ST::px(wx0, lane, p);
+                    const size_t pix = (size_t)ST::py(wy0, lane, p) * iW + ST::px(wx0, lane, p);
                     oc[pix] = C0[p] + T[p] * vb0;
-                    oc[HW + pix] = C1[p] + T[p] * vb1;
-                    oc[2 * HW + pix] = C2[p] + T[p] * vb2;
+                    oc[vhw + pix] = C1[p] + T[p] * vb1;
+                    oc[2 * vhw + pix] = C2[p] + T[p] * vb2;
                     od[pix] = D[p];
                     oa[pix] = 1.f - T[p];
                     nc[pix] = last[p];
@@ -396,20 +398,20 @@ render_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
                   const float *__restrict__ bg, float *__restrict__ out_color,
                   float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
                   float *__restrict__ final_T) {
-    render_fwd_body<PPL, U, LAZY, false>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, 0);
+    render_fwd_body<PPL, U, LAZY, false>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, nullptr);
 }
 
 // the batched forward: the default sub-tile shape <1,1> only (8 CTAs per SM, as render_fwd_kernel<1,1>)
 template <bool LAZY>
 __global__ void __launch_bounds__(kRenderThreads, 8)
-render_views_fwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+render_views_fwd_kernel(const __grid_constant__ ViewTable vt, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
                   const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
                   int two_ended, int sms, CostOrder co, unsigned *__restrict__ lazy_note,
                   const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
                   const float *__restrict__ bg, float *__restrict__ out_color,
                   float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
-                  float *__restrict__ final_T, int tiles_view) {
-    render_fwd_body<1, 1, LAZY, true>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, tiles_view);
+                  float *__restrict__ final_T) {
+    render_fwd_body<1, 1, LAZY, true>(0, 0, 0, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, &vt);
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -441,7 +443,7 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                   const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
                   const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
                   const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
-                  float *__restrict__ grad_rec, int tiles_view) {
+                  float *__restrict__ grad_rec, const ViewTable *vt) {
     using ST = SubTile<PPL>;
     using SM = BwdSmem<PPL>;
     constexpr int kPix = SM::kPix;
@@ -486,16 +488,18 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
         const unsigned ot = by_cost ? item / 8u : item / ST::kPerTile;
         const int tile = (int)__ldcg(tile_order + ot), sub = (int)(by_cost ? item % 8u : item % ST::kPerTile);
         const uint2 range = __ldcg(order_ranges + ot);
-        int v = 0, lt = tile;
-        if (VIEWS) { v = tile / tiles_view; lt = tile - v * tiles_view; }
-        const int tx = lt % gx, ty = lt / gx;
+        int v = 0, lt = tile, iW = W, iH = H, igx = gx;          // VIEWS: the item's view and its size
+        if constexpr (VIEWS) { v = view_of_tile(*vt, tile); lt = tile - vt->tile_off[v]; iW = vt->W[v]; iH = vt->H[v]; igx = vt->gx[v]; }
+        const int tx = lt % igx, ty = lt / igx;
         const int wx0 = ST::x0(tx, sub), wy0 = ST::y0(ty, sub);
         const int wx1 = wx0 + ST::kW - 1, wy1 = wy0 + ST::kH - 1;
         const float *vfT = final_T, *vgC = gC, *vgD = gD, *vgA = gA;
         const unsigned *vnc = n_contrib;
-        if (VIEWS) {
+        size_t iHW = HW;
+        if constexpr (VIEWS) {
             b0 = __ldg(bg + 3 * v); b1 = __ldg(bg + 3 * v + 1); b2 = __ldg(bg + 3 * v + 2);
-            const size_t vb = (size_t)v * HW;
+            const size_t vb = (size_t)vt->pix_off[v];
+            iHW = (size_t)iH * iW;
             vfT += vb; vnc += vb;
             if (gC) vgC += 3 * vb;
             if (gD) vgD += vb;
@@ -510,11 +514,11 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
             const int x = ST::px(wx0, lane, p), y = ST::py(wy0, lane, p);
             fx[p] = (float)x; fy[p] = (float)y;
             gc0[p] = 0.f; gc1[p] = 0.f; gc2[p] = 0.f; gd[p] = 0.f; ga[p] = 0.f; T[p] = 1.f; last[p] = 0;
-            if ((x < W) && (y < H)) {
-                const size_t pix = (size_t)y * W + x;
+            if ((x < iW) && (y < iH)) {
+                const size_t pix = (size_t)y * iW + x;
                 last[p] = __ldcg(vnc + pix);
                 T[p] = __ldcg(vfT + pix);
-                if (gC) { gc0[p] = __ldg(vgC + pix); gc1[p] = __ldg(vgC + HW + pix); gc2[p] = __ldg(vgC + 2 * HW + pix); }
+                if (gC) { gc0[p] = __ldg(vgC + pix); gc1[p] = __ldg(vgC + iHW + pix); gc2[p] = __ldg(vgC + 2 * iHW + pix); }
                 if (gD) gd[p] = __ldg(vgD + pix);
                 if (gA) ga[p] = __ldg(vgA + pix);
             }
@@ -712,20 +716,20 @@ render_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order,
                   const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
                   const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
                   float *__restrict__ grad_rec) {
-    render_bwd_body<PPL, U, LAZY, ROWSUM, false>(H, W, gx, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, 0);
+    render_bwd_body<PPL, U, LAZY, ROWSUM, false>(H, W, gx, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, nullptr);
 }
 
 // the batched backward: the default sub-tile shape <1,2> with the per-row step 2 only
 template <bool LAZY>
 __global__ void __launch_bounds__(kRenderThreads)
-render_views_bwd_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
+render_views_bwd_kernel(const __grid_constant__ ViewTable vt, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
                   unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
                   const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ lazy_note,
                   const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
                   const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
                   const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
-                  float *__restrict__ grad_rec, int tiles_view) {
-    render_bwd_body<1, 2, LAZY, true, true>(H, W, gx, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, tiles_view);
+                  float *__restrict__ grad_rec) {
+    render_bwd_body<1, 2, LAZY, true, true>(0, 0, 0, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, &vt);
 }
 
 }  // namespace dgr

@@ -14,6 +14,7 @@
 
 #include <mutex>
 #include <unordered_map>
+#include <vector>
 
 #include "../../include/dgr_b200.h"
 
@@ -195,9 +196,10 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
     return g;
 }
 
-// ---- batched cameras (DgrViews, dgr_views_*): one cloud, V same-size views per call ----------------------------------------
+// ---- batched cameras (DgrViews, dgr_views_*): one cloud, V same-size views per call; dgr_views_mixed_*: a size per view ------
 struct ViewsState {
     DgrViews s;
+    std::vector<int32_t> hw;         // mixed sizes: [V,2] (height, width) on the host; empty for the same-size call
     DgrGaussians g;
     Tensor tanfov, bg, view, proj, campos;
     Tensor means3D, opac;
@@ -215,6 +217,15 @@ uint64_t views_hint_key(int dev, int64_t P, int H, int W, int V) {
     return h;
 }
 
+std::unordered_map<uint64_t, Hint> g_views_mixed_hints; // keyed by (device, P, the views' sizes), apart from the other hints
+uint64_t views_mixed_hint_key(int dev, int64_t P, const std::vector<int32_t> &hw) {
+    uint64_t h = 1469598103934665603ull;
+    auto mix = [&](uint64_t x) { h ^= x; h *= 1099511628211ull; };
+    mix((uint64_t)dev); mix((uint64_t)P); mix((uint64_t)hw.size());
+    for (int32_t x : hw) mix((uint64_t)(uint32_t)x);
+    return h;
+}
+
 // instance capacity the binning buffer may be sized for: the 32-bit positions of the kernels, and half the free device memory
 int64_t views_capacity_ceiling(int64_t V, int64_t H, int64_t W) {
     size_t free_b = 0, total_b = 0;
@@ -226,11 +237,14 @@ int64_t views_capacity_ceiling(int64_t V, int64_t H, int64_t W) {
     return ceil;
 }
 
+// hw: empty = the same-size call at H x W; else the [V,2] sizes of the mixed call (H, W unused), flat outputs
 std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
-views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov, const Tensor &bg,
-              const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh, const Tensor &opac,
-              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double scale_modifier, int64_t sh_degree, bool debug,
+                   const Tensor &tanfov, const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D,
+                   const Tensor &sh, const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
     auto st = std::make_shared<ViewsState>();
+    st->hw = hw;
+    const bool mixed = !hw.empty();
     st->means3D = dev_f32(means3D, "means3D");
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     st->device = st->means3D.get_device();
@@ -238,6 +252,7 @@ views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bo
     st->tanfov = dev_f32(tanfov, "tanfov"); st->bg = dev_f32(bg, "bg"); st->view = dev_f32(view, "viewmatrix");
     st->proj = dev_f32(proj, "projmatrix"); st->campos = dev_f32(campos, "campos");
     const int64_t V = st->bg.size(0);
+    TORCH_CHECK_VALUE(!mixed || (int64_t)hw.size() == 2 * V, "image_hw must have dimensions (num_views, 2)");
     TORCH_CHECK_VALUE(st->tanfov.numel() == 2 * V && st->bg.numel() == 3 * V && st->view.numel() == 16 * V && st->proj.numel() == 16 * V &&
                       st->campos.numel() == 3 * V, "per-view tanfov [V,2], bg / campos [V,3], viewmatrix / projmatrix [V,16] expected");
     st->sh = dev_f32(sh, "shs"); st->scales = dev_f32(scales, "scales"); st->rots = dev_f32(rots, "rotations");
@@ -264,17 +279,34 @@ views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bo
                          fptr(st->sh_rest), activations ? 1 : 0};
     const auto f32 = st->means3D.options();
     const auto u8 = f32.dtype(torch::kUInt8);
-    Tensor color = torch::empty({V, 3, H, W}, f32), depth = torch::empty({V, 1, H, W}, f32), alpha = torch::empty({V, 1, H, W}, f32);
+    Tensor color, depth, alpha;
+    const int32_t *ihw = mixed ? hw.data() : nullptr;
+    if (mixed) {                     // flat: view v's blocks at pixel pix_off[v] (include/dgr_b200.h)
+        int64_t pix = 0;
+        for (int64_t v = 0; v < V; v++) pix += (int64_t)hw[2 * v] * hw[2 * v + 1];
+        color = torch::empty({3 * pix}, f32); depth = torch::empty({pix}, f32); alpha = torch::empty({pix}, f32);
+    } else {
+        color = torch::empty({V, 3, H, W}, f32); depth = torch::empty({V, 1, H, W}, f32); alpha = torch::empty({V, 1, H, W}, f32);
+    }
     st->radii = torch::empty({V, P}, f32.dtype(torch::kInt32));
-    st->geom = torch::empty({(int64_t)dgr_views_geom_bytes((int32_t)V, (int32_t)P, (int32_t)H, (int32_t)W)}, u8);
-    st->image = torch::empty({(int64_t)dgr_views_image_bytes((int32_t)V, (int32_t)H, (int32_t)W)}, u8);
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
-    check(dgr_views_forward_preprocess(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), stream));
+    if (mixed) {
+        const size_t gb = dgr_views_mixed_geom_bytes((int32_t)V, (int32_t)P, ihw), ib = dgr_views_mixed_image_bytes((int32_t)V, ihw);
+        st->geom = torch::empty({(int64_t)std::max<size_t>(gb, 1)}, u8);
+        st->image = torch::empty({(int64_t)std::max<size_t>(ib, 1)}, u8);
+        check(dgr_views_mixed_forward_preprocess(&st->s, ihw, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(),
+                                                 stream));
+    } else {
+        st->geom = torch::empty({(int64_t)dgr_views_geom_bytes((int32_t)V, (int32_t)P, (int32_t)H, (int32_t)W)}, u8);
+        st->image = torch::empty({(int64_t)dgr_views_image_bytes((int32_t)V, (int32_t)H, (int32_t)W)}, u8);
+        check(dgr_views_forward_preprocess(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), stream));
+    }
     DgrImages out{color.data_ptr<float>(), depth.data_ptr<float>(), alpha.data_ptr<float>(), st->radii.data_ptr<int32_t>()};
     const int64_t ceiling = views_capacity_ceiling(V, H, W);
     Hint hint{std::min<int64_t>(std::max<int64_t>(65536, 16 * P * V), ceiling), true};
-    const uint64_t key = views_hint_key(st->device, P, (int)H, (int)W, (int)V);
-    { std::lock_guard<std::mutex> lk(g_mu); auto it = g_views_hints.find(key); if (it != g_views_hints.end()) hint = it->second; }
+    auto &hints = mixed ? g_views_mixed_hints : g_views_hints;
+    const uint64_t key = mixed ? views_mixed_hint_key(st->device, P, hw) : views_hint_key(st->device, P, (int)H, (int)W, (int)V);
+    { std::lock_guard<std::mutex> lk(g_mu); auto it = hints.find(key); if (it != hints.end()) hint = it->second; }
     SyncObjs &so = sync_objs(st->device);
     int64_t cap = hint.cap, n_inst = 0, n_big = 0;
     bool big = hint.big;
@@ -283,9 +315,13 @@ views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bo
         st->binning = torch::empty({(int64_t)dgr_views_binning_bytes((uint64_t)cap, (int32_t)V, (int32_t)H, (int32_t)W)}, u8);
         const uint64_t ticket = ++so.ticket;
         volatile uint64_t *cnt = reinterpret_cast<volatile uint64_t *>(so.counts.data_ptr<int64_t>());
-        check(dgr_views_forward_render(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
-                                       (big ? DGR_FLAG_BIG_TILES : 0) | rerun, reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>()), ticket,
-                                       nullptr, stream));
+        uint64_t *counts = reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>());
+        if (mixed)
+            check(dgr_views_mixed_forward_render(&st->s, ihw, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(),
+                                                 &out, (big ? DGR_FLAG_BIG_TILES : 0) | rerun, counts, ticket, nullptr, stream));
+        else
+            check(dgr_views_forward_render(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
+                                           (big ? DGR_FLAG_BIG_TILES : 0) | rerun, counts, ticket, nullptr, stream));
         {
             pybind11::gil_scoped_release nogil;
             uint64_t spins = 0;
@@ -307,14 +343,36 @@ views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bo
         rerun = DGR_FLAG_RERUN;
     }
     { std::lock_guard<std::mutex> lk(g_mu);
-      g_views_hints[key] = Hint{std::min<int64_t>(std::max<int64_t>((int64_t)(n_inst * 1.25) + 4096, 65536), 0xfffffffell), n_big > 0}; }
+      hints[key] = Hint{std::min<int64_t>(std::max<int64_t>((int64_t)(n_inst * 1.25) + 4096, 65536), 0xfffffffell), n_big > 0}; }
     st->capacity = cap; st->n_inst = n_inst; st->staging = (int32_t)so.counts.data_ptr<int64_t>()[3];
     return {color, st->radii, depth, alpha, st};
 }
 
-// grads: (means3D, means2D [V,P,3], shs | features_dc, opacities, scales, rotations, features_rest); the per-Gaussian ones summed over views
-std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
-                                   bool accumulate, const std::vector<OptTensor> &out) {
+std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
+views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov, const Tensor &bg,
+              const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh, const Tensor &opac,
+              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+    return views_forward_impl(H, W, {}, scale_modifier, sh_degree, debug, tanfov, bg, view, proj, campos, means3D, sh, opac, scales, rots,
+                              sh_rest, activations);
+}
+
+// views of different sizes: image_hw = [V,2] (height, width); color [sum 3 H_v W_v], depth / alpha [sum H_v W_v] (flat)
+std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
+views_mixed_forward(const std::vector<int32_t> &image_hw, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov,
+                    const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh,
+                    const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+    TORCH_CHECK_VALUE(!image_hw.empty() && image_hw.size() % 2 == 0, "image_hw must have dimensions (num_views, 2)");
+    int64_t H = 0, W = 0;                                    // the capacity ceiling's bytes per instance do not depend on the size
+    for (size_t i = 0; i < image_hw.size(); i += 2) { H = std::max<int64_t>(H, image_hw[i]); W = std::max<int64_t>(W, image_hw[i + 1]); }
+    return views_forward_impl(H, W, image_hw, scale_modifier, sh_degree, debug, tanfov, bg, view, proj, campos, means3D, sh, opac, scales,
+                              rots, sh_rest, activations);
+}
+
+// grads: (means3D, means2D [V,P,3], shs | features_dc, opacities, scales, rotations, features_rest); the per-Gaussian ones summed over views.
+// Mixed sizes only: the densification statistics of the views in stats_views.
+std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
+                                        bool accumulate, const std::vector<OptTensor> &out, const OptTensor &xyz_gradient_accum,
+                                        const OptTensor &denom, const OptTensor &max_radii2D, uint64_t stats_views) {
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     const int64_t P = st->g.P, M = st->g.M, V = st->s.V;
     const auto f32 = st->means3D.options();
@@ -331,11 +389,21 @@ std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const 
     pick(4, true, {P, 3}); pick(5, true, {P, 4}); pick(6, act && st->sh_rest.has_value(), {P, M - 1, 3});
     auto gp = [&](size_t i) -> float * { return g[i].defined() && g[i].numel() > 0 ? g[i].data_ptr<float>() : nullptr; };
     DgrImageGrads gin{fptr(c), fptr(d), fptr(a)};
-    DgrGaussianGrads gout{gp(0), gp(1), gp(2), nullptr, gp(3), gp(4), gp(5), nullptr, accumulate ? 1 : 0, gp(6), nullptr, nullptr, nullptr, nullptr};
+    DgrGaussianGrads gout{gp(0), gp(1), gp(2), nullptr, gp(3), gp(4), gp(5), nullptr, accumulate ? 1 : 0, gp(6),
+                          fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D), nullptr};
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
-    check(dgr_views_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
-                             st->radii.data_ptr<int32_t>(), &gin, &gout, stream));
+    if (!st->hw.empty())
+        check(dgr_views_mixed_backward(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
+                                       st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views, stream));
+    else
+        check(dgr_views_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
+                                 st->radii.data_ptr<int32_t>(), &gin, &gout, stream));
     return g;
+}
+
+std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
+                                   bool accumulate, const std::vector<OptTensor> &out) {
+    return views_backward_impl(st, gC, gD, gA, accumulate, out, c10::nullopt, c10::nullopt, c10::nullopt, 0);
 }
 
 }  // namespace
@@ -354,6 +422,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("views_forward", &views_forward, "both forward stages of the batched-camera call through the C ABI");
     m.def("views_backward", &views_backward, "backward of the batched-camera call through the C ABI", pybind11::arg("state"),
           pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"));
+    m.def("views_mixed_forward", &views_mixed_forward, "both forward stages of the batched call with a size per view through the C ABI");
+    m.def("views_mixed_backward", &views_backward_impl, "backward of the batched call with a size per view through the C ABI",
+          pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"),
+          pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"), pybind11::arg("denom"), pybind11::arg("max_radii2D"),
+          pybind11::arg("stats_views"));
+    m.def("set_views_mixed_hint", [](int dev, int64_t P, const std::vector<int32_t> &hw, int64_t cap, bool big) {
+        std::lock_guard<std::mutex> lk(g_mu); g_views_mixed_hints[views_mixed_hint_key(dev, P, hw)] = Hint{cap, big}; });
+    m.def("get_views_mixed_hint", [](int dev, int64_t P, const std::vector<int32_t> &hw) -> pybind11::object {
+        std::lock_guard<std::mutex> lk(g_mu);
+        auto it = g_views_mixed_hints.find(views_mixed_hint_key(dev, P, hw));
+        if (it == g_views_mixed_hints.end()) return pybind11::none();
+        return pybind11::make_tuple(it->second.cap, it->second.big); });
     m.def("set_views_hint", [](int dev, int64_t P, int H, int W, int V, int64_t cap, bool big) {
         std::lock_guard<std::mutex> lk(g_mu); g_views_hints[views_hint_key(dev, P, H, W, V)] = Hint{cap, big}; });
     m.def("get_views_hint", [](int dev, int64_t P, int H, int W, int V) -> pybind11::object {

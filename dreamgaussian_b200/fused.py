@@ -137,3 +137,47 @@ def rasterize_views_raw(settings_list, xyz, means2D, features_dc, features_rest,
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), xyz.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
     return _RasterizeViewsRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, settings_list)
+
+
+class _RasterizeViewsMixedRaw(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xyz, means2D, features_dc, features_rest, opacity_raw, scaling_raw, rotation_raw, settings_list, stats, stats_mask):
+        xyz = _r._dev_f32(xyz, "xyz")
+        dc = _r._dev_f32(features_dc, "features_dc")
+        rest = _r._opt(features_rest, "features_rest")
+        if rest is not None and rest.numel() == 0:
+            rest = None
+        op, sc, rot = _r._dev_f32(opacity_raw, "opacity"), _r._dev_f32(scaling_raw, "scaling"), _r._dev_f32(rotation_raw, "rotation")
+        color, radii, depth, alpha, state = _r.views_forward_impl(settings_list, xyz, dc, op, sc, rot, sh_rest=rest, activations=True,
+                                                                  mixed=True)
+        ctx.state, ctx.stats, ctx.stats_mask = state, (stats if stats_mask else None), stats_mask
+        ctx.mark_non_differentiable(radii)
+        return color, radii, depth, alpha
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
+        state = ctx.state
+        # as _RasterizeRaw: the statistics describe the forward, a retain_graph / second backward must not count its views twice
+        if getattr(state, "stats_applied", False):
+            ctx.stats = None
+        state.stats_applied = True
+        d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot = _r._views_grads(state, grad_color, grad_depth, grad_alpha, raw=True, stats=ctx.stats,
+                                                                        stats_views=ctx.stats_mask)
+        return d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, None
+
+
+def rasterize_views_mixed_raw(settings_list, xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, stats=None,
+                              stats_views=()):
+    """rasterize_views_mixed (rasterizer.py) for GaussianModel's RAW parameters: one cloud, cameras of any image sizes, the
+    activations applied in the kernels and the gradients summed over the views with respect to the raw tensors.  Returns
+    (colors, radii, depths, alphas) as rasterize_views_mixed.  `stats` (DensifyStats) is updated during the backward for the views
+    listed in `stats_views` (indices into settings_list), in view order, as one fused single-view render of each would update it;
+    once per forward."""
+    settings_list = _r._check_views_mixed_settings(settings_list)
+    if means2D is not None and tuple(means2D.shape) != (len(settings_list), xyz.shape[0], 3):
+        raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
+    mask = _r._stats_mask(stats_views, len(settings_list))
+    color, radii, depth, alpha = _RasterizeViewsMixedRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation,
+                                                               settings_list, stats if mask else None, mask)
+    colors, depths, alphas = _r.split_views(settings_list, color, depth, alpha)
+    return colors, radii, depths, alphas

@@ -374,19 +374,51 @@ def _views_capacity_ceiling(lib, dev, V, H, W):
     return min(_MAX_CAPACITY, max(65536, (free // 2) // per))
 
 
-def _check_views_settings(settings_list):
+def get_views_mixed_capacity_hint(device_index, P, sizes):
+    """Instance-capacity hint of the mixed-size batched call, keyed by the tuple of (height, width) sizes."""
+    sizes = tuple((int(h), int(w)) for h, w in sizes)
+    if _FAST is not None:
+        return _FAST.get_views_mixed_hint(device_index, P, [x for hw in sizes for x in hw])
+    return _CAPACITY_HINT.get(("views_mixed", device_index, P, sizes))
+
+
+def set_views_mixed_capacity_hint(device_index, P, sizes, cap, big):
+    sizes = tuple((int(h), int(w)) for h, w in sizes)
+    if _FAST is not None:
+        _FAST.set_views_mixed_hint(device_index, P, [x for hw in sizes for x in hw], cap, big)
+    else:
+        _CAPACITY_HINT[("views_mixed", device_index, P, sizes)] = (cap, big)
+
+
+def _check_views_settings(settings_list, fields=("image_height", "image_width", "sh_degree", "scale_modifier"), what="rasterize_views"):
     settings_list = list(settings_list)
     if not settings_list:
-        raise ValueError("rasterize_views needs at least one camera")
+        raise ValueError("%s needs at least one camera" % what)
     if len(settings_list) > _lib.VIEWS_MAX:
-        raise ValueError("rasterize_views takes at most %d cameras per call, got %d" % (_lib.VIEWS_MAX, len(settings_list)))
+        raise ValueError("%s takes at most %d cameras per call, got %d" % (what, _lib.VIEWS_MAX, len(settings_list)))
     s0 = settings_list[0]
     for i, s in enumerate(settings_list[1:], 1):
-        for f in ("image_height", "image_width", "sh_degree", "scale_modifier"):
+        for f in fields:
             if getattr(s, f) != getattr(s0, f):
-                raise ValueError("rasterize_views: every camera of a batch must share %s (camera 0 has %r, camera %d has %r)"
-                                 % (f, getattr(s0, f), i, getattr(s, f)))
+                raise ValueError("%s: every camera of a batch must share %s (camera 0 has %r, camera %d has %r)"
+                                 % (what, f, getattr(s0, f), i, getattr(s, f)))
     return settings_list
+
+
+def _check_views_mixed_settings(settings_list):
+    """The cameras of a mixed-size batch: any image sizes, one sh_degree and scale_modifier."""
+    return _check_views_settings(settings_list, ("sh_degree", "scale_modifier"), "rasterize_views_mixed")
+
+
+def _stats_mask(stats_views, V):
+    """View indices -> the stats_views bit mask of dgr_views_mixed_backward."""
+    mask = 0
+    for v in stats_views:
+        v = int(v)
+        if v < 0 or v >= V:
+            raise ValueError("stats_views: view %d is not in the batch of %d views" % (v, V))
+        mask |= 1 << v
+    return mask
 
 
 def _views_cameras(settings_list, dev):
@@ -402,13 +434,16 @@ def _views_cameras(settings_list, dev):
 class _Views:
     """ctypes views of one batched call's cameras + inputs (keeps the tensors alive)."""
 
-    def __init__(self, settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False):
+    def __init__(self, settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False, mixed=False):
         dev = means3D.device
         s0 = settings_list[0]
         V = len(settings_list)
         self.tanfov, self.bg, self.view, self.proj, self.campos = _views_cameras(settings_list, dev)
         self.keep = [self.bg, self.view, self.proj, self.campos, self.tanfov]
         self.V, self.H, self.W = V, int(s0.image_height), int(s0.image_width)
+        # mixed sizes: the host [V,2] (height, width) array the dgr_views_mixed_* calls take
+        self.sizes = tuple((int(s.image_height), int(s.image_width)) for s in settings_list)
+        self.hw = (ctypes.c_int32 * (2 * V))(*[x for hw in self.sizes for x in hw]) if mixed else None
         self.settings = _lib.DgrViews(V, self.H, self.W, float(s0.scale_modifier), int(s0.sh_degree), int(bool(s0.debug)),
                                       _ptr(self.tanfov), _ptr(self.bg), _ptr(self.view), _ptr(self.proj), _ptr(self.campos))
         # the per-Gaussian checks of the single-view call (shapes, raw-parameter layout)
@@ -419,49 +454,73 @@ class _Views:
 
 class ViewsState:
     """Everything one batched forward leaves behind for its backward."""
-    __slots__ = ("views", "capacity", "staging", "num_rendered", "geom", "binning", "image", "radii", "tensors", "fast")
+    __slots__ = ("views", "capacity", "staging", "num_rendered", "geom", "binning", "image", "radii", "tensors", "fast", "mixed",
+                 "stats_applied")
 
 
-def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False):
+def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False, mixed=False):
     """Both forward stages of the batched call through the C ABI; inputs are validated CUDA float32 tensors.
     Returns (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W], ViewsState).  Same speculative-capacity
-    protocol as forward_impl, with hints keyed by (device, P, H, W, V); the compiled host layer when it is loaded."""
+    protocol as forward_impl, with hints keyed by (device, P, H, W, V); the compiled host layer when it is loaded.
+    mixed=True: every camera has its own image size (dgr_views_mixed_*); color [sum 3 H_v W_v], depth / alpha [sum H_v W_v]
+    are flat, view v's blocks one after the other, and the hints are keyed by (device, P, the sizes)."""
     lib = _lib.load()
     dev = means3D.device
     if _FAST is not None:
         s0 = settings_list[0]
         with torch.cuda.device(dev):
             cams = _views_cameras(settings_list, dev)
-        color, radii, depth, alpha, cst = _FAST.views_forward(
-            int(s0.image_height), int(s0.image_width), float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams,
-            means3D, sh, opacities, scales, rotations, sh_rest, bool(activations))
+        if mixed:
+            hw = [int(x) for s in settings_list for x in (s.image_height, s.image_width)]
+            color, radii, depth, alpha, cst = _FAST.views_mixed_forward(
+                hw, float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams, means3D, sh, opacities, scales, rotations, sh_rest,
+                bool(activations))
+        else:
+            color, radii, depth, alpha, cst = _FAST.views_forward(
+                int(s0.image_height), int(s0.image_width), float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams,
+                means3D, sh, opacities, scales, rotations, sh_rest, bool(activations))
         state = ViewsState()
         state.fast, state.capacity, state.num_rendered, state.radii = cst, cst.capacity, cst.num_rendered, radii
         state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
+        state.mixed = mixed
         return color, radii, depth, alpha, state
     with torch.cuda.device(dev):
-        vw = _Views(settings_list, means3D, sh, opacities, scales, rotations, sh_rest, activations)
+        vw = _Views(settings_list, means3D, sh, opacities, scales, rotations, sh_rest, activations, mixed=mixed)
         V, H, W, P = vw.V, vw.H, vw.W, vw.P
         u8 = dict(dtype=torch.uint8, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
-        color, depth, alpha = torch.empty((V, 3, H, W), **f32), torch.empty((V, 1, H, W), **f32), torch.empty((V, 1, H, W), **f32)
+        if mixed:
+            pix = sum(h * w for h, w in vw.sizes)
+            color, depth, alpha = torch.empty((3 * pix,), **f32), torch.empty((pix,), **f32), torch.empty((pix,), **f32)
+        else:
+            color, depth, alpha = torch.empty((V, 3, H, W), **f32), torch.empty((V, 1, H, W), **f32), torch.empty((V, 1, H, W), **f32)
         radii = torch.empty((V, P), dtype=torch.int32, device=dev)
-        geom = torch.empty((lib.dgr_views_geom_bytes(V, P, H, W),), **u8)
-        image = torch.empty((lib.dgr_views_image_bytes(V, H, W),), **u8)
         n_host, event = _host_sync_objects(dev)
         st = _stream_ptr(dev)
-        _lib.check(lib.dgr_views_forward_preprocess(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(image),
-                                                    _ptr(radii), st))
+        if mixed:
+            geom = torch.empty((max(1, lib.dgr_views_mixed_geom_bytes(V, P, vw.hw)),), **u8)
+            image = torch.empty((max(1, lib.dgr_views_mixed_image_bytes(V, vw.hw)),), **u8)
+            _lib.check(lib.dgr_views_mixed_forward_preprocess(ctypes.byref(vw.settings), vw.hw, ctypes.byref(vw.gaussians), _ptr(geom),
+                                                              _ptr(image), _ptr(radii), st))
+            key = ("views_mixed", dev.index, P, vw.sizes)
+        else:
+            geom = torch.empty((lib.dgr_views_geom_bytes(V, P, H, W),), **u8)
+            image = torch.empty((lib.dgr_views_image_bytes(V, H, W),), **u8)
+            _lib.check(lib.dgr_views_forward_preprocess(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(image),
+                                                        _ptr(radii), st))
+            key = ("views", dev.index, P, H, W, V)
         out = _lib.DgrImages(_ptr(color), _ptr(depth), _ptr(alpha), _ptr(radii))
-        key = ("views", dev.index, P, H, W, V)
         ceiling = _views_capacity_ceiling(lib, dev, V, H, W)
         cap, big = _CAPACITY_HINT.get(key, (min(max(65536, 16 * P * V), ceiling), True))
         rerun = 0
         while True:
             binning = torch.empty((lib.dgr_views_binning_bytes(cap, V, H, W),), **u8)
-            _lib.check(lib.dgr_views_forward_render(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(binning),
-                                                    ctypes.c_uint64(cap), _ptr(image), ctypes.byref(out), (1 if big else 0) | rerun,
-                                                    ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event, st))
+            args = (ctypes.byref(vw.gaussians), _ptr(geom), _ptr(binning), ctypes.c_uint64(cap), _ptr(image), ctypes.byref(out),
+                    (1 if big else 0) | rerun, ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event, st)
+            if mixed:
+                _lib.check(lib.dgr_views_mixed_forward_render(ctypes.byref(vw.settings), vw.hw, *args))
+            else:
+                _lib.check(lib.dgr_views_forward_render(ctypes.byref(vw.settings), *args))
             _lib.check(lib.dgr_event_synchronize(event))
             n_inst, n_big = int(n_host[0]), int(n_host[1])
             if n_inst <= cap and (big or n_big == 0):
@@ -473,7 +532,7 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
             rerun = 2                                   # DGR_FLAG_RERUN
         _CAPACITY_HINT[key] = (min(max(int(n_inst * 1.25) + 4096, 65536), _MAX_CAPACITY), n_big > 0)
     state = ViewsState()
-    state.fast = None
+    state.fast, state.mixed = None, mixed
     state.views, state.capacity, state.staging, state.num_rendered = vw, cap, int(n_host[3]), n_inst
     state.geom, state.binning, state.image, state.radii = geom, binning, image, radii
     state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
@@ -481,12 +540,17 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
 
 
 def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot,
-                        accumulate=False, d_sh_rest=None):
+                        accumulate=False, d_sh_rest=None, densify=None, stats_views=0):
     """Backward of a batched forward: the per-Gaussian gradients are the sums over the views (written, or added with
-    accumulate); d_means2D is per view, [V,P,3]."""
+    accumulate); d_means2D is per view, [V,P,3].  Mixed-size forwards only: densify = (xyz_gradient_accum, denom, max_radii2D)
+    float32 [P] tensors (any may be None), updated for the views whose bit is set in the stats_views mask."""
     if state.fast is not None:
-        _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate),
-                             [d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest])
+        outs = [d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest]
+        if state.mixed:
+            _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs, *(densify or (None, None, None)),
+                                       int(stats_views))
+        else:
+            _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs)
         return
     lib = _lib.load()
     vw = state.views
@@ -494,16 +558,26 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
     with torch.cuda.device(dev):
         gin = _lib.DgrImageGrads(_ptr(grad_color), _ptr(grad_depth), _ptr(grad_alpha))
         gout = _lib.DgrGaussianGrads(_ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), None, _ptr(d_opac), _ptr(d_scales), _ptr(d_rot),
-                                     None, 1 if accumulate else 0, _ptr(d_sh_rest), None, None, None, None)
-        _lib.check(lib.dgr_views_backward(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning),
-                                          ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii),
-                                          ctypes.byref(gin), ctypes.byref(gout), _stream_ptr(dev)))
+                                     None, 1 if accumulate else 0, _ptr(d_sh_rest),
+                                     *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), None)
+        common = (ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning), ctypes.c_uint64(state.capacity), state.staging,
+                  _ptr(state.image), _ptr(state.radii), ctypes.byref(gin), ctypes.byref(gout))
+        if state.mixed:
+            _lib.check(lib.dgr_views_mixed_backward(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views), _stream_ptr(dev)))
+        else:
+            _lib.check(lib.dgr_views_backward(ctypes.byref(vw.settings), *common, _stream_ptr(dev)))
 
 
-def _views_grads(state, grad_color, grad_depth, grad_alpha, raw):
-    """-> (means3D, means2D [V,P,3], shs | features_dc, features_rest, opacities, scales, rotations) gradients."""
+def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, stats_views=0):
+    """-> (means3D, means2D [V,P,3], shs | features_dc, features_rest, opacities, scales, rotations) gradients.
+    stats (DensifyStats) / stats_views (bit mask): the densification statistics of a mixed-size forward."""
+    densify = stats.as_tuple() if stats is not None else None
     if state.fast is not None:
-        g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [])       # undefined -> None
+        if state.mixed:
+            g = _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *(densify or (None, None, None)),
+                                           int(stats_views) if densify is not None else 0)
+        else:
+            g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [])       # undefined -> None
         return g[0], g[1], g[2], g[6], g[3], g[4], g[5]
     means3D, sh, opacities, scales, rotations, sh_rest = state.tensors
     vw = state.views
@@ -516,7 +590,8 @@ def _views_grads(state, grad_color, grad_depth, grad_alpha, raw):
     d_sh = torch.empty((P, 1 if raw else M, 3), **f32)
     d_rest = torch.empty(sh_rest.shape, **f32) if (raw and sh_rest is not None) else None
     d_scales, d_rot = torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
-    views_backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest=d_rest)
+    views_backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest=d_rest, densify=densify,
+                        stats_views=stats_views if densify is not None else 0)
     return d_means3D, d_means2D, d_sh, d_rest, d_opac, d_scales, d_rot
 
 
@@ -560,3 +635,48 @@ class GaussianViewsRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs, scales, rotations):
         return rasterize_views(self.settings_list, means3D, means2D, opacities, shs, scales, rotations)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Batched cameras of different image sizes: one cloud, V views, each with its own size (include/dgr_b200.h, dgr_views_mixed_*).
+# ---------------------------------------------------------------------------------------------------------------------------
+def split_views(settings_list, color, depth, alpha):
+    """The flat outputs of a mixed-size call -> per-view lists: colour [3,H_v,W_v], depth / alpha [1,H_v,W_v] (views of the flat
+    tensors, so gradients flow back into them)."""
+    colors, depths, alphas, off = [], [], [], 0
+    for s in settings_list:
+        h, w = int(s.image_height), int(s.image_width)
+        colors.append(color.narrow(0, 3 * off, 3 * h * w).view(3, h, w))
+        depths.append(depth.narrow(0, off, h * w).view(1, h, w))
+        alphas.append(alpha.narrow(0, off, h * w).view(1, h, w))
+        off += h * w
+    return colors, depths, alphas
+
+
+class _RasterizeViewsMixed(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list):
+        means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
+        sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
+        color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, mixed=True)
+        ctx.state = state
+        ctx.mark_non_differentiable(radii)
+        return color, radii, depth, alpha
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
+        d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=False)
+        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None
+
+
+def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scales, rotations):
+    """rasterize_views for cameras of DIFFERENT image sizes (at most 64, one sh_degree / scale_modifier): one batched forward
+    and one batched backward.  Returns (colors, radii, depths, alphas): colors a list of [3,H_v,W_v], depths / alphas lists of
+    [1,H_v,W_v] (views of one flat tensor each), radii int32 [V,P]; view v equals what GaussianRasterizer returns for camera v.
+    The gradients of means3D / shs / opacities / scales / rotations are summed over the views; means2D is [V,P,3] or None."""
+    settings_list = _check_views_mixed_settings(settings_list)
+    if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
+        raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
+    color, radii, depth, alpha = _RasterizeViewsMixed.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list)
+    colors, depths, alphas = split_views(settings_list, color, depth, alpha)
+    return colors, radii, depths, alphas

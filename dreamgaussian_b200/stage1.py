@@ -332,11 +332,16 @@ def synthetic_rgba(size):
 class Stage1Trainer:
     """main.py:182-287 train_step, guidance stubbed.  `fused=True`: FusedGaussianRasterizer + fused Adam (rows f1 + f2);
     `fused=False`: the reference's formulation through this library's plain op — torch activations + torch.cat, the three
-    torch statistic updates, torch.optim.Adam-style per-tensor updates — the baseline tools/stage1_bench.py times."""
+    torch statistic updates, torch.optim.Adam-style per-tensor updates — the baseline tools/stage1_bench.py times.
+    `batched=True` (needs fused=True): the known and the novel view of a step are ONE mixed-size batched render
+    (fused.rasterize_views_mixed_raw) with one forward and one backward, the statistics taken from the novel view only; same
+    cameras, rng draws and loss terms as the default path, whose gradient summation order it does not share."""
 
-    def __init__(self, cfg: Stage1Config = Stage1Config(), optim: OptimConfig = OptimConfig(), device="cuda", fused=True):
+    def __init__(self, cfg: Stage1Config = Stage1Config(), optim: OptimConfig = OptimConfig(), device="cuda", fused=True, batched=False):
         from . import scene
-        self.cfg, self.device, self.fused = cfg, torch.device(device), fused
+        if batched and not fused:
+            raise ValueError("Stage1Trainer: batched=True needs fused=True (the batched call takes the raw parameters)")
+        self.cfg, self.device, self.fused, self.batched = cfg, torch.device(device), fused, batched
         self.rng = np.random.default_rng(cfg.seed)
         self.scene = scene
         cloud = scene.make_cloud(cfg.num_pts, cfg.sh_degree, seed=cfg.seed, anisotropic=False, sigma=1.0)      # positions only
@@ -383,34 +388,62 @@ class Stage1Trainer:
         g.update_learning_rate(self.step)
         g.zero_grad()
         densify_window = cfg.density_start_iter <= self.step <= cfg.density_end_iter
-        # known view (main.py:196-208)
-        out = self.render(self.fixed_cam, track_stats=False)
-        loss = 10000 * step_ratio * torch.nn.functional.mse_loss(out["image"].unsqueeze(0), self.input_img)
-        loss = loss + 1000 * step_ratio * torch.nn.functional.mse_loss(out["alpha"].unsqueeze(0), self.input_mask)
-        # novel view (main.py:210-240); the statistics come from this LAST render of the step (main.py:278-281)
-        res = 128 if step_ratio < 0.3 else (256 if step_ratio < 0.6 else 512)
-        min_ver = max(min(cfg.min_ver, cfg.min_ver - cfg.elevation), -80 - cfg.elevation)
-        max_ver = min(max(cfg.max_ver, cfg.max_ver - cfg.elevation), 80 - cfg.elevation)
-        ver, hor = int(self.rng.integers(min_ver, max_ver)), int(self.rng.integers(-180, 180))
-        bg = (1.0, 1.0, 1.0) if self.rng.random() > cfg.invert_bg_prob else (0.0, 0.0, 0.0)
-        out = self.render(self._settings(cfg.elevation + ver, hor, cfg.radius, res, bg), track_stats=densify_window)
-        loss = loss + cfg.lambda_zero123 * self.guidance.train_step(out["image"].unsqueeze(0), [ver], [hor], [0], step_ratio=step_ratio,
-                                                                    default_elevation=cfg.elevation)
+        if self.batched:
+            loss = self._batched_loss(step_ratio, densify_window)
+        else:
+            loss = self._loss(step_ratio, densify_window)
         loss.backward()
         g.optimizer_step()
         if densify_window:
             if not self.fused:          # the reference's three torch updates (main.py:279-281, gs_renderer.py:625-627)
                 with torch.no_grad():
-                    vis, radii, st = out["visibility_filter"], out["radii"], g.stats
+                    vis, radii, st = self._last["visibility_filter"], self._last["radii"], g.stats
                     st.max_radii2D[vis] = torch.max(st.max_radii2D[vis], radii[vis].float())
-                    st.xyz_gradient_accum[vis] += torch.norm(out["viewspace_points"].grad[vis, :2], dim=-1)
+                    st.xyz_gradient_accum[vis] += torch.norm(self._last["viewspace_points"].grad[vis, :2], dim=-1)
                     st.denom[vis] += 1
             if self.step % cfg.densification_interval == 0:
                 g.densify_and_prune(cfg.densify_grad_threshold, min_opacity=0.01, extent=4, max_screen_size=1)
             if self.step % cfg.opacity_reset_interval == 0:          # main.py:285-286 (700 > 500 iterations in image.yaml)
                 g.reset_opacity()
+        self._last = None
         self.losses.append(loss.detach())
         return loss
+
+    def _novel_camera(self, step_ratio):
+        """The novel view's camera (main.py:210-226): its resolution by step_ratio, then ver, hor, bg drawn from the rng."""
+        cfg = self.cfg
+        res = 128 if step_ratio < 0.3 else (256 if step_ratio < 0.6 else 512)
+        min_ver = max(min(cfg.min_ver, cfg.min_ver - cfg.elevation), -80 - cfg.elevation)
+        max_ver = min(max(cfg.max_ver, cfg.max_ver - cfg.elevation), 80 - cfg.elevation)
+        ver, hor = int(self.rng.integers(min_ver, max_ver)), int(self.rng.integers(-180, 180))
+        bg = (1.0, 1.0, 1.0) if self.rng.random() > cfg.invert_bg_prob else (0.0, 0.0, 0.0)
+        return self._settings(cfg.elevation + ver, hor, cfg.radius, res, bg), ver, hor
+
+    def _batched_loss(self, step_ratio, densify_window):
+        """The loss of the step from ONE batched render of [known view, novel view] (sizes ref_size and res)."""
+        from .fused import rasterize_views_mixed_raw
+        cfg, g = self.cfg, self.gaussians
+        novel, ver, hor = self._novel_camera(step_ratio)
+        colors, radii, depths, alphas = rasterize_views_mixed_raw(
+            [self.fixed_cam, novel], g._xyz, None, g._features_dc, g._features_rest, g._opacity, g._scaling, g._rotation,
+            stats=g.stats if densify_window else None, stats_views=(1,) if densify_window else ())
+        loss = 10000 * step_ratio * torch.nn.functional.mse_loss(colors[0].clamp(0, 1).unsqueeze(0), self.input_img)
+        loss = loss + 1000 * step_ratio * torch.nn.functional.mse_loss(alphas[0].unsqueeze(0), self.input_mask)
+        return loss + cfg.lambda_zero123 * self.guidance.train_step(colors[1].clamp(0, 1).unsqueeze(0), [ver], [hor], [0], step_ratio=step_ratio,
+                                                                     default_elevation=cfg.elevation)
+
+    def _loss(self, step_ratio, densify_window):
+        cfg = self.cfg
+        # known view (main.py:196-208)
+        out = self.render(self.fixed_cam, track_stats=False)
+        loss = 10000 * step_ratio * torch.nn.functional.mse_loss(out["image"].unsqueeze(0), self.input_img)
+        loss = loss + 1000 * step_ratio * torch.nn.functional.mse_loss(out["alpha"].unsqueeze(0), self.input_mask)
+        # novel view (main.py:210-240); the statistics come from this LAST render of the step (main.py:278-281)
+        novel, ver, hor = self._novel_camera(step_ratio)
+        out = self.render(novel, track_stats=densify_window)
+        self._last = out
+        return loss + cfg.lambda_zero123 * self.guidance.train_step(out["image"].unsqueeze(0), [ver], [hor], [0], step_ratio=step_ratio,
+                                                                    default_elevation=cfg.elevation)
 
     def train(self, iters=None):
         for _ in range(iters or self.cfg.iters):

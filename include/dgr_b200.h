@@ -227,6 +227,32 @@ int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom, con
                        int32_t staging, const void *image, const int32_t *radii, const DgrImageGrads *gin,
                        const DgrGaussianGrads *gout, void *stream);
 
+/* == Batched cameras of DIFFERENT image sizes: the batched call above with a size per view ==
+ * image_hw: HOST array [V,2] of (height, width); DgrViews.image_height / image_width are ignored.  Everything else of DgrViews
+ * and of the same-size call holds (cameras, shared SH degree and scale modifier, inputs, protocol, kernels).  Outputs are FLAT:
+ * with pix_off[v] = sum over u < v of H_u W_u, view v's colour is the contiguous [3,H_v,W_v] block at float 3 pix_off[v] of
+ * DgrImages.color, and its depth / alpha the [H_v,W_v] blocks at float pix_off[v] of depth / alpha (the image gradients of the
+ * backward use the same layout); radii [V,P] and dL_dmeans2D [V,P,3] as above.  A batch whose sizes are all equal computes what
+ * the same-size call computes, bit for bit, with the same scratch sizes.
+ * Densification statistics: the backward updates DgrGaussianGrads.xyz_gradient_accum / denom / max_radii2D (float [P], any may
+ * be NULL) for the views whose bit is set in stats_views (bit v = view v), in ascending view order, each with the single-view
+ * rule (dgr_backward) for that view's means2D gradient and radii: what one single-view backward per selected view would leave.
+ * Refused before any device work: image_hw NULL, a size <= 0 or > 65535, more than 51200 tiles (16x16) in the batch, V outside
+ * 1..DGR_VIEWS_MAX, V x P > DGR_VIEWS_MAX_RECORDS, a stats_views bit at or above V, stats_views != 0 with no statistic buffer or
+ * a statistic buffer with stats_views == 0, colors_precomp / cov3D_precomp, and DgrPeerPush.
+ * Scratch: dgr_views_mixed_geom_bytes / dgr_views_mixed_image_bytes (0 for sizes the calls refuse); binning as
+ * dgr_views_binning_bytes. */
+size_t dgr_views_mixed_geom_bytes(int32_t V, int32_t P, const int32_t *image_hw);
+size_t dgr_views_mixed_image_bytes(int32_t V, const int32_t *image_hw);
+int dgr_views_mixed_forward_preprocess(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, void *image,
+                                       int32_t *radii, void *stream);
+int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, void *binning,
+                                   uint64_t capacity_instances, void *image, const DgrImages *out, int32_t flags, uint64_t *counts_host,
+                                   uint64_t ticket, void *count_ready_event, void *stream);
+int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, const void *binning,
+                             uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii,
+                             const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views, void *stream);
+
 /* Multi-GPU (view-sharded data parallelism, SURVEY.md §8e): all-reduce(sum) of the flat float32 gradient buffer over
  * NVLink with this library's own kernel.  The buffer lives in symmetric memory: peer_ptrs[w] (HOST array of `world` device
  * addresses) is rank w's copy mapped into this process; multicast_ptr, if non-zero, is the NVSwitch multicast address of
