@@ -136,7 +136,6 @@ constexpr size_t kMaxTileSmem = 200 * 1024;      // tile-histogram rows live in 
 
 // tuning knobs of dgr_set_tuning bits 24-26 (atomics, like the ones further down)
 std::atomic<int> g_stage_fwd{1}, g_stage_bwd{1};   // per-Gaussian kernels: inputs staged through shared memory by bulk TMA (dgr_preprocess.cuh)
-std::atomic<int> g_sort_fine{0};               // per-tile sort with 2048 instead of 1024 depth buckets (A/B, bit 28)
 std::atomic<int> g_rowsum{1};                  // backward render, step 2: per-row form of the dy moments (dgr_render.cuh, ROWSUM)
 
 // Can the per-Gaussian kernels stage their inputs with bulk TMA (dgr_preprocess.cuh)?  SH + scale / rotation inputs, every base
@@ -254,7 +253,6 @@ std::atomic<int> g_lazy{0};            // record staging of the render kernels: 
 std::atomic<int> g_cta_fwd{0}, g_cta_bwd{0};   // persistent CTAs per SM of the render kernels (0 = as many as fit)
 
 using SmS = SortSmem<kSortSmallThreads, kSortSmallCap, kSortSmallBuckets>;
-using SmSF = SortSmem<kSortSmallThreads, kSortSmallCap, kSortSmallBucketsFine>;
 using SmB = SortSmem<kSortBigThreads, kSortBigCap, kSortBigBuckets>;
 
 // Per-DEVICE launch state: cudaFuncSetAttribute (dynamic shared memory above 48 KB) and the occupancy-derived persistent
@@ -284,7 +282,6 @@ DevInfo *dev_info() {
     cudaError_t e = cudaFuncSetAttribute(emit_instances_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTileSmem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(emit_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTileSmem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tile_sort_gather_kernel<kSortSmallBuckets>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmS::bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tile_sort_gather_kernel<kSortSmallBucketsFine>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmSF::bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tile_sort_gather_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmB::bytes);
     if (e != cudaSuccess) { fail((int)e, "cudaFuncSetAttribute", cudaGetErrorString(e)); return nullptr; }
     d.ready = true;
@@ -343,17 +340,10 @@ int launch_tile_sorts(DevInfo *dv, const char *image, const ImageLayout &IL, int
                       unsigned long long *keys, const Rec *rec, unsigned *ids, Rec *recs, int debug, cudaStream_t st) {
     const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
     const uint2 *oranges = reinterpret_cast<const uint2 *>(image + IL.off_oranges);
-    if (g_sort_fine.load()) {
-        const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBucketsFine>, kSortSmallThreads, SmSF::bytes));
-        DGR_KERNEL("tile_sort_gather", st, debug,
-                   launch_k(tile_sort_gather_kernel<kSortSmallBucketsFine>, dim3(sort_grid), dim3(kSortSmallThreads), SmSF::bytes, st, true, work,
-                            oranges, keys, rec, ids, recs, lazy ? 0 : 1));
-    } else {
-        const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBuckets>, kSortSmallThreads, SmS::bytes));
-        DGR_KERNEL("tile_sort_gather", st, debug,
-                   launch_k(tile_sort_gather_kernel<kSortSmallBuckets>, dim3(sort_grid), dim3(kSortSmallThreads), SmS::bytes, st, true, work,
-                            oranges, keys, rec, ids, recs, lazy ? 0 : 1));
-    }
+    const int sort_grid = min(tiles, persistent_grid(dv, tile_sort_gather_kernel<kSortSmallBuckets>, kSortSmallThreads, SmS::bytes));
+    DGR_KERNEL("tile_sort_gather", st, debug,
+               launch_k(tile_sort_gather_kernel<kSortSmallBuckets>, dim3(sort_grid), dim3(kSortSmallThreads), SmS::bytes, st, true, work,
+                        oranges, keys, rec, ids, recs, lazy ? 0 : 1));
     if (big_tiles)
         DGR_KERNEL("tile_sort_gather_big", st, debug,
                    launch_k(tile_sort_gather_big_kernel, dim3(dv->big_grid), dim3(kSortBigThreads), SmB::bytes, st, true, work,
@@ -419,7 +409,6 @@ int dgr_set_tuning(int ppl_fwd, int ppl_bwd, int tile_order) {
     g_lazy = (tile_order >> 22) & 3;                    // bits 22-23: record staging 0 = auto, 1 = always the sorted copy, 2 = always by id
     g_stage_fwd = (tile_order >> 24) & 1 ? 0 : 1;       // bit 24 / 25: per-Gaussian forward / backward kernel reads its inputs with
     g_stage_bwd = (tile_order >> 25) & 1 ? 0 : 1;       // per-thread global loads instead of bulk-TMA staging (A/B switch)
-    g_sort_fine = (tile_order >> 28) & 1;               // bit 28: per-tile sort with 2048 depth buckets (A/B switch)
     g_rowsum = (tile_order >> 26) & 1 ? 0 : 1;          // bit 26: backward render step 2 in the per-pixel form (A/B switch; <1,2> non-lazy only)
     return 0;
 }

@@ -454,28 +454,42 @@ __device__ __forceinline__ void sort_gather_tile(const uint2 r, unsigned long lo
         }
     }
     __syncthreads();
-    // rank inside the bucket with the full key, write id + record to the final position
+    // rank inside the bucket with the full key, write the id to the final position; then the warp moves the records of its
+    // (up to) 32 keys together: 96 16-byte pieces, piece c = part c % 3 of key c / 3.  So one 128-bit load or store touches
+    // about 11 records, not the 32 scattered ones of a lane per record, and the stores, whose positions are a near-permutation
+    // of a contiguous range, coalesce.
     const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-    for (int i = tid; i < n; i += THREADS) {
-        const unsigned long long kk = B[i];
-        const float d = __uint_as_float((unsigned)(kk >> 32));
-        const int bk = min(nb - 1, (int)((d - dmin) * scale));
-        const int s = (int)start[bk], e = (int)start[bk + 1];
-        int rank = 0;
-        for (int j = s; j < e; j++) rank += (B[j] < kk) ? 1 : 0;
-        const unsigned gid = (unsigned)(kk & 0xffffffffull);
-        const size_t pos = (size_t)r.x + s + rank;
-        ids_sorted[pos] = gid;
+    for (int i0 = tid - lane; i0 < n; i0 += THREADS) {                     // warp-uniform: the shuffles need every lane
+        const int i = i0 + lane;
+        unsigned gid = 0u;
+        int pos = -1;                                                        // -1: no key for this lane
+        if (i < n) {
+            const unsigned long long kk = B[i];
+            const float d = __uint_as_float((unsigned)(kk >> 32));
+            const int bk = min(nb - 1, (int)((d - dmin) * scale));
+            const int s = (int)start[bk], e = (int)start[bk + 1];
+            int rank = 0;
+            for (int j = s; j < e; j++) rank += (B[j] < kk) ? 1 : 0;
+            gid = (unsigned)(kk & 0xffffffffull);
+            pos = s + rank;
+            ids_sorted[(size_t)r.x + pos] = gid;
+        }
         if (gather) {
-            const Rec *src = rec + gid;
-            const float4 g0 = ldg_f4_hint(&src->q0, pol_keep), g1 = ldg_f4_hint(&src->q1, pol_keep), g2 = ldg_f4_hint(&src->q2, pol_keep);
-            Rec *dst = rec_sorted + pos;
-            stg_f4_hint(&dst->q0, g0, pol_stream); stg_f4_hint(&dst->q1, g1, pol_stream); stg_f4_hint(&dst->q2, g2, pol_stream);
+#pragma unroll
+            for (int m = 0; m < 3; m++) {
+                const int c = m * 32 + lane, k = c / 3, part = c - 3 * k;
+                const unsigned g = __shfl_sync(0xffffffffu, gid, k);
+                const int p = __shfl_sync(0xffffffffu, pos, k);
+                if (p >= 0) {
+                    const float4 v = ldg_f4_hint(reinterpret_cast<const float4 *>(rec + g) + part, pol_keep);
+                    stg_f4_hint(reinterpret_cast<float4 *>(rec_sorted + r.x + p) + part, v, pol_stream);
+                }
+            }
         }
     }
 }
 
-constexpr int kSortSmallThreads = 512, kSortSmallBuckets = 1024, kSortSmallBucketsFine = 2048;   // (Fine: A/B, dgr_set_tuning bit 28)
+constexpr int kSortSmallThreads = 512, kSortSmallBuckets = 1024;
 constexpr int kSortBigThreads = 1024, kSortBigCap = 12288, kSortBigBuckets = 2048;     // 96 KB of keys + 16 KB of bucket tables
 
 // Persistent grid over the NON-EMPTY tiles in issue order (heaviest first, dealt round-robin to the CTAs): CTA c sorts entries

@@ -163,7 +163,6 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom, 
  *                each warp's 32 contiguous Gaussians through shared memory with bulk TMA (A/B switch; the staged path needs
  *                SH + scale / rotation inputs and 16-byte aligned base pointers and is otherwise not taken anyway)
  *   bit 26       step 2 of the backward render kernel in its per-pixel form (A/B switch; default sub-tile shape only)
- *   bit 28       per-tile depth sort with 2048 instead of 1024 buckets (A/B switch)
  * the other bits are accepted and ignored.  The knobs may change between a forward and its backward: each call reads them when
  * it launches, and the backward stages its records the way its forward did (counts_host[3] -> dgr_backward's `staging`). */
 int dgr_set_tuning(int ppl_fwd, int ppl_bwd, int tile_order);
@@ -197,7 +196,7 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom, const 
  * Kernel shapes: the batched render kernels are the default sub-tile shapes only (forward 8x4 pixels per warp, one hit at a time;
  * backward 8x4 with two hits together and the per-row step 2): dgr_set_tuning's pixels-per-lane, hits-together and bit 26 do not
  * apply to them.  The scheduling knobs (cost order, two-ended queue, CTAs per SM, PDL), record staging (bits 22-23), input
- * staging of the forward (bit 24) and the sort buckets (bit 28) do. */
+ * staging of the forward (bit 24) do. */
 #define DGR_VIEWS_MAX 64
 #define DGR_VIEWS_MAX_RECORDS 2147483647ll
 typedef struct DgrViews {
