@@ -85,6 +85,7 @@ EXPORTS = (
     "dgr_views_forward_render", "dgr_views_backward",
     "dgr_views_mixed_geom_bytes", "dgr_views_mixed_image_bytes", "dgr_views_mixed_forward_preprocess",
     "dgr_views_mixed_forward_render", "dgr_views_mixed_backward",
+    "dgr_det_scratch_bytes", "dgr_backward_det", "dgr_views_backward_det", "dgr_views_mixed_backward_det",
 )
 
 _lib = None
@@ -193,6 +194,15 @@ def load():
     lib.dgr_views_mixed_backward.restype = ctypes.c_int
     lib.dgr_views_mixed_backward.argtypes = [ctypes.POINTER(DgrViews), hw, ctypes.POINTER(DgrGaussians), vp, vp, u64, i32, vp, vp,
                                              ctypes.POINTER(DgrImageGrads), ctypes.POINTER(DgrGaussianGrads), u64, vp]
+    # the deterministic backward: the counterpart's arguments + (det_scratch, det_scratch_bytes, instances)
+    lib.dgr_det_scratch_bytes.restype = ctypes.c_size_t
+    lib.dgr_det_scratch_bytes.argtypes = [u64, ctypes.c_int64]
+    lib.dgr_backward_det.restype = ctypes.c_int
+    lib.dgr_backward_det.argtypes = list(lib.dgr_backward.argtypes[:-1]) + [vp, u64, u64, vp]
+    lib.dgr_views_backward_det.restype = ctypes.c_int
+    lib.dgr_views_backward_det.argtypes = list(lib.dgr_views_backward.argtypes[:-1]) + [vp, u64, u64, vp]
+    lib.dgr_views_mixed_backward_det.restype = ctypes.c_int
+    lib.dgr_views_mixed_backward_det.argtypes = list(lib.dgr_views_mixed_backward.argtypes[:-1]) + [vp, u64, u64, vp]
     if lib.dgr_abi_version() != ABI_VERSION:
         raise RuntimeError("libdgr_b200.so ABI version mismatch")
     _lib = lib

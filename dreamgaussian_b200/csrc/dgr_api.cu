@@ -20,6 +20,7 @@
 #include "dgr_binning.cuh"
 #include "dgr_collective.cuh"
 #include "dgr_densify.cuh"
+#include "dgr_det.cuh"
 #include "dgr_knn.cuh"
 #include "dgr_fields.cuh"
 #include "dgr_optim.cuh"
@@ -365,6 +366,79 @@ CostOrder cost_order(const char *image, const ImageLayout &IL, int tiles, int bw
     }
     return co;
 }
+
+// ---- the deterministic backward (dgr_*_backward_det, dgr_det.cuh) --------------------------------------------------------------
+struct DetArgs { void *scratch; uint64_t bytes; uint64_t instances; };
+
+// the refusals of the deterministic calls on top of their counterparts' (before any device work)
+int check_det(const DetArgs &d, const DgrGaussianGrads *gout, uint64_t capacity, long long records) {
+    if (gout->push) return fail(-2, "deterministic backward: DgrPeerPush is not supported");
+    if (d.instances > capacity) return fail(-1, "deterministic backward: instances above capacity_instances (pass the last stage-2 run's count)");
+    if (!d.scratch) return fail(-1, "deterministic backward: det_scratch is NULL");
+    if (d.bytes < DetLayout(d.instances, records).total)
+        return fail(-1, "deterministic backward: det_scratch is smaller than dgr_det_scratch_bytes(instances, records)");
+    return 0;
+}
+
+// Everything between the backward's memset and its per-Gaussian kernel: masked counts -> exclusive scan (goff) -> render_bwd_det ->
+// det_moments_gather, which leaves grad_rec as the default render kernel would, summed in a fixed order.  vt = NULL: single view.
+int det_render(DevInfo *dv, const DetArgs &d, long long R, int H, int W, int gx, const ViewTable *vt, int tiles, const char *image,
+               const ImageLayout &IL, char *geom, const GeomLayout &GL, const char *binning, const BinningLayout &BL, bool lazy,
+               const float *bg, const DgrImageGrads *gin, float *grad_rec, int debug, cudaStream_t st) {
+    if (debug) {                                     // debug: the caller's instance count against the forward's own (a host sync)
+        unsigned long long n_fwd = 0;
+        DGR_CUDA(cudaMemcpyAsync(&n_fwd, geom + offsetof(GeomHeader, n_inst), sizeof(n_fwd), cudaMemcpyDeviceToHost, st));
+        DGR_CUDA(cudaStreamSynchronize(st));
+        if (n_fwd != d.instances)
+            return fail(-1, "deterministic backward: instances differs from the forward's instance count (pass the last stage-2 run's count)");
+    }
+    const DetLayout DL(d.instances, R);
+    char *det = (char *)d.scratch;
+    float *mom = reinterpret_cast<float *>(det + DL.off_mom);
+    unsigned *goff = reinterpret_cast<unsigned *>(det + DL.off_goff), *sums = reinterpret_cast<unsigned *>(det + DL.off_sums);
+    const unsigned *touched = reinterpret_cast<const unsigned *>(geom + GL.off_touched);
+    if (d.instances > 0) {
+        prof_begin("det_memset", st);
+        const cudaError_t e = cudaMemsetAsync(mom, 0, (size_t)d.instances * kGradRecFloats * 4, st);
+        prof_end(st);
+        if (e != cudaSuccess) return fail((int)e, "det_memset", cudaGetErrorString(e));
+    }
+    const unsigned nb = (unsigned)((R + 255) / 256);
+    DGR_KERNEL("det_counts", st, debug, launch_k(det_counts_kernel, dim3(nb), dim3(256), 0, st, false, R, touched, goff));
+    DGR_KERNEL("det_scan_sums", st, debug, launch_k(knn_scan_sums_kernel, dim3((unsigned)DL.nblk), dim3(1024), 0, st, false,
+                                                     (const unsigned *)goff, (size_t)R, sums));
+    DGR_KERNEL("det_scan_top", st, debug, launch_k(knn_scan_top_kernel, dim3(1), dim3(1024), 0, st, false, sums, DL.nblk));
+    DGR_KERNEL("det_scan_apply", st, debug, launch_k(knn_scan_apply_kernel, dim3((unsigned)DL.nblk), dim3(1024), 0, st, false,
+                                                      goff, (size_t)R, (const unsigned *)sums));
+    const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
+    unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
+    const unsigned *order = reinterpret_cast<const unsigned *>(image + IL.off_order);
+    const uint2 *oranges = reinterpret_cast<const uint2 *>(image + IL.off_oranges);
+    const Rec *recs = reinterpret_cast<const Rec *>(binning + BL.off_rec), *rec = reinterpret_cast<const Rec *>(geom + GL.off_rec);
+    const unsigned *ids = reinterpret_cast<const unsigned *>(binning + BL.off_ids);
+    const float *fT = reinterpret_cast<const float *>(image + IL.off_finalT);
+    const unsigned *nc = reinterpret_cast<const unsigned *>(image + IL.off_ncontrib);
+    const unsigned long long n_slots = d.instances;
+    const size_t smem = sizeof(DetSmem);
+    auto launch = [&](auto kernel, const char *name, auto... head) -> int {
+        int grid = min(persistent_grid(dv, kernel, kDetThreads, smem), tiles);
+        if (g_cta_bwd.load() > 0) grid = min(grid, g_cta_bwd.load() * dv->sms);
+        DGR_KERNEL(name, st, debug, launch_k(kernel, dim3((unsigned)grid), dim3(kDetThreads), smem, st, true, head..., order, oranges,
+                                             &work->n_nonempty, bwd_next, recs, rec, ids, (const unsigned *)goff, n_slots, bg, fT, nc,
+                                             gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, mom));
+        return 0;
+    };
+    int e = 0;
+    if (d.instances == 0) {}                         // nothing binned: no instance row to fill (the gather flags any touched record)
+    else if (vt) e = lazy ? launch(render_views_bwd_det_kernel<true>, "render_views_bwd_det", *vt)
+                     : launch(render_views_bwd_det_kernel<false>, "render_views_bwd_det", *vt);
+    else e = lazy ? launch(render_bwd_det_kernel<true>, "render_bwd_det", H, W, gx)
+                  : launch(render_bwd_det_kernel<false>, "render_bwd_det", H, W, gx);
+    if (e) return e;
+    DGR_KERNEL("det_moments_gather", st, debug, launch_k(det_moments_gather_kernel, dim3(nb), dim3(256), 0, st, true, R, touched,
+                                                         (const unsigned *)goff, (const float *)mom, n_slots, grad_rec));
+    return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -536,16 +610,17 @@ static int flat_segs(int32_t n_seg, const int64_t *seg_off, const int32_t *seg_s
     return 0;
 }
 
-int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
-                 int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
-                 const DgrGaussianGrads *gout, void *stream) {
-    NvtxRange nvtx_("dgr_backward");
-    (void)out_alpha;
+// dgr_backward (det = NULL) and dgr_backward_det
+static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
+                           int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                           const DgrGaussianGrads *gout, const DetArgs *det, void *stream) {
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
     if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
         return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
+    if (det)
+        if (int e = check_det(*det, gout, capacity, g->P)) return e;
     if (g->P == 0) return 0;
     if (!radii) return fail(-1, "radii is NULL");
     if (int e = check_push(gout->push, g->P)) return e;
@@ -560,7 +635,12 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
     float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
     // one memset: the work counter of the persistent backward render kernel + the per-Gaussian moment accumulators
     DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * kGradRecFloats * 4, st));
-    if (binning && capacity > 0) {
+    if (det && binning && capacity > 0) {
+        DevInfo *dv = dev_info();
+        if (!dv) return -1;
+        if (int e = det_render(dv, *det, g->P, H, W, IL.gx, nullptr, tiles, image, IL, geom, GL, binning, BL, staging == DGR_STAGING_BY_ID,
+                               s->bg, gin, grad_rec, s->debug, st)) return e;
+    } else if (binning && capacity > 0) {
         DevInfo *dv = dev_info();
         if (!dv) return -1;
         const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
@@ -607,6 +687,25 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
     }
     DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, st));
     return 0;
+}
+
+int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
+                 int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                 const DgrGaussianGrads *gout, void *stream) {
+    NvtxRange nvtx_("dgr_backward");
+    (void)out_alpha;
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, stream);
+}
+
+size_t dgr_det_scratch_bytes(uint64_t instances, int64_t records) { return DetLayout(instances, records).total; }
+
+int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
+                     int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                     const DgrGaussianGrads *gout, void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, void *stream) {
+    NvtxRange nvtx_("dgr_backward_det");
+    (void)out_alpha;
+    const DetArgs det{det_scratch, det_scratch_bytes, instances};
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, stream);
 }
 
 }  // extern "C"
@@ -821,7 +920,9 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
 
 int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                    int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views,
-                   void *stream) {
+                   const DetArgs *det, void *stream) {
+    if (det)
+        if (int e = check_det(*det, gout, capacity, (long long)g->P * s->V)) return e;
     if (g->P == 0) return 0;
     if (!radii) return fail(-1, "radii is NULL");
     cudaStream_t st = (cudaStream_t)stream;
@@ -833,7 +934,12 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
     const int tiles = b.tiles;
     float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
     DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * s->V * kGradRecFloats * 4, st));
-    if (binning && capacity > 0) {
+    if (det && binning && capacity > 0) {
+        DevInfo *dv = dev_info();
+        if (!dv) return -1;
+        if (int e = det_render(dv, *det, (long long)g->P * s->V, 0, 0, 0, &b.vt, tiles, image, IL, geom, GL, binning, BL,
+                               staging == DGR_STAGING_BY_ID, s->bg, gin, grad_rec, s->debug, st)) return e;
+    } else if (binning && capacity > 0) {
         DevInfo *dv = dev_info();
         if (!dv) return -1;
         const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
@@ -889,9 +995,9 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
                         count_ready_event, stream);
 }
 
-int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
-                       const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
-    NvtxRange nvtx_("dgr_views_backward");
+static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                               const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
+                               const DetArgs *det, void *stream) {
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -900,7 +1006,21 @@ int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, c
     if (gout->xyz_gradient_accum || gout->denom || gout->max_radii2D)
         return fail(-2, "views: the fused densification statistics are not supported by the batched call");
     if (int e = check_views_grads(gout)) return e;
-    return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, stream);
+    return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, det, stream);
+}
+
+int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                       const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
+    NvtxRange nvtx_("dgr_views_backward");
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, stream);
+}
+
+int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                           const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
+                           void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, void *stream) {
+    NvtxRange nvtx_("dgr_views_backward_det");
+    const DetArgs det{det_scratch, det_scratch_bytes, instances};
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, stream);
 }
 
 // ---- views of different sizes: image_hw = [V,2] (height, width) on the host ------------------------------------------------------
@@ -936,10 +1056,9 @@ int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, c
                         count_ready_event, stream);
 }
 
-int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
-                             uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                             const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
-    NvtxRange nvtx_("dgr_views_mixed_backward");
+static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
+                                uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, void *stream) {
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -953,7 +1072,23 @@ int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const D
         return fail(-1, "views mixed: a densification statistic buffer is set but stats_views is 0");
     if (int e = check_views_grads(gout)) return e;
     return views_backward(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout,
-                          stats_views, stream);
+                          stats_views, det, stream);
+}
+
+int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
+                             uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                             const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_backward");
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, stream);
+}
+
+int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
+                                 uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                                 const DgrGaussianGrads *gout, uint64_t stats_views, void *det_scratch, uint64_t det_scratch_bytes,
+                                 uint64_t instances, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_backward_det");
+    const DetArgs det{det_scratch, det_scratch_bytes, instances};
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, stream);
 }
 
 }  // extern "C"

@@ -54,6 +54,12 @@ struct State {                       // what one forward leaves behind for its b
     int device = 0;
 };
 
+// scratch of the deterministic backward (dgr_*_backward_det), taken when torch.use_deterministic_algorithms(True) is in effect
+// (warn_only included) at the time the backward runs
+Tensor det_scratch(int64_t instances, int64_t records, const torch::TensorOptions &like) {
+    return torch::empty({(int64_t)dgr_det_scratch_bytes((uint64_t)instances, records)}, like.dtype(torch::kUInt8));
+}
+
 struct Hint { int64_t cap; bool big; };
 std::mutex g_mu;
 std::unordered_map<uint64_t, Hint> g_hints;
@@ -191,6 +197,13 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D),
                           reinterpret_cast<const DgrPeerPush *>(push_addr)};      // host struct kept alive by the caller (0 = none)
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
+    if (at::globalContext().deterministicAlgorithms()) {
+        Tensor det = det_scratch(st->n_inst, P, f32);
+        check(dgr_backward_det(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
+                               st->image.data_ptr(), st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, det.data_ptr(),
+                               (uint64_t)det.numel(), (uint64_t)st->n_inst, stream));
+        return g;
+    }
     check(dgr_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
                        st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, stream));
     return g;
@@ -392,6 +405,18 @@ std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, c
     DgrGaussianGrads gout{gp(0), gp(1), gp(2), nullptr, gp(3), gp(4), gp(5), nullptr, accumulate ? 1 : 0, gp(6),
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D), nullptr};
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
+    if (at::globalContext().deterministicAlgorithms()) {
+        Tensor det = det_scratch(st->n_inst, P * V, f32);
+        const uint64_t n = (uint64_t)st->n_inst, bytes = (uint64_t)det.numel();
+        if (!st->hw.empty())
+            check(dgr_views_mixed_backward_det(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
+                                               st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views,
+                                               det.data_ptr(), bytes, n, stream));
+        else
+            check(dgr_views_backward_det(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
+                                         st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, det.data_ptr(), bytes, n, stream));
+        return g;
+    }
     if (!st->hw.empty())
         check(dgr_views_mixed_backward(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
                                        st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views, stream));

@@ -179,7 +179,9 @@ class ViewShardedRasterizer:
                 rs, params["means3D"], params["shs"], None, params["opacities"], params["scales"], params["rotations"], None)
             # the backward of the LAST local view also delivers the rows other ranks own (local sum of all this rank's views)
             # to their owners' staging areas: the reduce-scatter half of the all-reduce rides on that kernel
-            last = fused and i == len(settings) - 1
+            # (not under torch.use_deterministic_algorithms: the deterministic backward takes no push, so the rows travel by
+            #  dgr_peer_push_flat after the last view instead, as for a rank without a view)
+            last = fused and i == len(settings) - 1 and not torch.are_deterministic_algorithms_enabled()
             _r.backward_impl(state, up[0], up[1], up[2], g["means3D"], g["means2D"], g["shs"], None, g["opacities"],
                              g["scales"], g["rotations"], None, accumulate=(i > 0), push=self._push if last else None)
             self._pushed = self._pushed or last

@@ -269,9 +269,24 @@ def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2
         gout = _lib.DgrGaussianGrads(_ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), _ptr(d_col), _ptr(d_opac), _ptr(d_scales),
                                      _ptr(d_rot), _ptr(d_cov), 1 if accumulate else 0, _ptr(d_sh_rest),
                                      *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), push_addr or None)
-        _lib.check(lib.dgr_backward(ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(state.geom), _ptr(state.binning),
-                                    ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii), _ptr(state.alpha),
-                                    ctypes.byref(gin), ctypes.byref(gout), _stream_ptr(dev)))
+        args = (ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(state.geom), _ptr(state.binning),
+                ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii), _ptr(state.alpha),
+                ctypes.byref(gin), ctypes.byref(gout))
+        if torch.are_deterministic_algorithms_enabled():
+            det = _det_scratch(lib, state.num_rendered, fr.P, dev)
+            _lib.check(lib.dgr_backward_det(*args, *_det_args(det, state.num_rendered), _stream_ptr(dev)))
+        else:
+            _lib.check(lib.dgr_backward(*args, _stream_ptr(dev)))
+
+
+def _det_scratch(lib, instances, records, dev):
+    """Scratch of the deterministic backward (dgr_*_backward_det), used when torch.use_deterministic_algorithms(True) is in effect
+    (warn_only included) at the time the backward runs."""
+    return torch.empty((lib.dgr_det_scratch_bytes(int(instances), int(records)),), dtype=torch.uint8, device=dev)
+
+
+def _det_args(det, instances):
+    return _ptr(det), ctypes.c_uint64(det.numel()), ctypes.c_uint64(int(instances))
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -562,6 +577,14 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
                                      *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), None)
         common = (ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning), ctypes.c_uint64(state.capacity), state.staging,
                   _ptr(state.image), _ptr(state.radii), ctypes.byref(gin), ctypes.byref(gout))
+        if torch.are_deterministic_algorithms_enabled():
+            det = _det_scratch(lib, state.num_rendered, vw.P * vw.V, dev)
+            if state.mixed:
+                _lib.check(lib.dgr_views_mixed_backward_det(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views),
+                                                            *_det_args(det, state.num_rendered), _stream_ptr(dev)))
+            else:
+                _lib.check(lib.dgr_views_backward_det(ctypes.byref(vw.settings), *common, *_det_args(det, state.num_rendered), _stream_ptr(dev)))
+            return
         if state.mixed:
             _lib.check(lib.dgr_views_mixed_backward(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views), _stream_ptr(dev)))
         else:

@@ -203,7 +203,7 @@ class GaussianModelB200:
             sel = (padded >= grad_threshold) & (scaling.max(dim=1).values > self.percent_dense * scene_extent)
             stds = scaling[sel].repeat(N, 1)
             if noise is None:
-                noise = torch.randn(stds.shape, device=stds.device)
+                noise = torch.randn(stds.shape, device=stds.device, generator=getattr(self, "noise_gen", None))
             samples = noise.to(stds) * stds
             rots = build_rotation(self.p["rotation"].detach()[sel]).repeat(N, 1, 1)
             new = dict(xyz=torch.bmm(rots, samples.unsqueeze(-1)).squeeze(-1) + self.p["xyz"].detach()[sel].repeat(N, 1),
@@ -240,7 +240,7 @@ class GaussianModelB200:
             n_keep, n_clone, n_sel, n_child = (int(x) for x in self._counts_host)
             n_out = n_keep + n_clone + 2 * n_child
             if noise is None:
-                noise = torch.randn((max(2 * n_sel, 1), 3), device=dev)
+                noise = torch.randn((max(2 * n_sel, 1), 3), device=dev, generator=getattr(self, "noise_gen", None))
             else:                                   # tests hand over the reference's draws: row = child * n_selected + rank
                 noise = noise.to(torch.empty((2 * n_sel, 3), device=dev)) if hasattr(noise, "to") else noise
             noise = noise.contiguous().float()
@@ -349,6 +349,9 @@ class Stage1Trainer:
         self.gaussians = GaussianModelB200(cfg.sh_degree)
         self.gaussians.fused_adam = fused
         self.gaussians.fused_densify = fused
+        # the split children's noise comes from the trainer's own generator: torch's default one is seeded differently in every
+        # process, so two runs from one seed would split differently at the first densification
+        self.gaussians.noise_gen = torch.Generator(device=self.device).manual_seed(cfg.seed)
         self.gaussians.create_from_points(cloud["means3D"], colors, spatial_lr_scale=10.0, device=device)      # gs_renderer.py:709
         self.gaussians.training_setup(optim)
         rgb, mask = synthetic_rgba(cfg.ref_size)

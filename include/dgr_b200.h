@@ -252,6 +252,40 @@ int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const D
                              uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii,
                              const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views, void *stream);
 
+/* == Deterministic backward: bit-reproducible gradients ==
+ * dgr_backward_det / dgr_views_backward_det / dgr_views_mixed_backward_det take the arguments of their counterparts plus
+ *   det_scratch        device scratch of at least dgr_det_scratch_bytes(instances, records) bytes (records = P, or V x P for the
+ *                      batched calls); its contents need not be initialised;
+ *   instances          the tile-instance count of the forward's LAST stage-2 run (counts_host[0]), at most capacity_instances.
+ * They compute what the counterpart computes, up to the order of the float additions that gather a Gaussian's gradient from the
+ * tiles it touches: here every such sum has a fixed order (within a tile: the 8x4-pixel sub-tiles in a fixed order; over the tiles:
+ * row-major within the Gaussian's tile rectangle) and no float atomic is used.  Guarantee: for the same inputs, forward scratch and
+ * upstream gradients on the same GPU model and library build, every output — the gradients, the per-view means2D gradients and
+ * the densification statistics — is bit-identical from call to call, whatever dgr_set_tuning's knobs (work order, CTAs per SM, PDL,
+ * pixels per lane, hits together), the record staging and the caller's thread or stream.  Not covered: a different library build or
+ * GPU model (ptxas chooses the fused multiply-adds), DgrGaussianGrads.accumulate onto non-deterministic values, and any
+ * cross-rank reduction of the multi-GPU path.
+ * Refused before any device work, each with its own dgr_last_error text: det_scratch NULL or smaller than dgr_det_scratch_bytes,
+ * instances > capacity_instances, DgrPeerPush, and everything the counterpart refuses.  With debug set (DgrSettings / DgrViews),
+ * `instances` is also compared with the forward's own count (one host synchronisation) and a mismatch is refused; without it, a
+ * count below the forward's leaves a NaN gradient row for every Gaussian whose tiles it does not cover.
+ * Cost: the counterpart's backward render kernel is replaced by render_bwd_det (one CTA per tile, a barrier per 32-record chunk)
+ * followed by det_moments_gather, and a scratch memset, a count kernel and three scan kernels run first; a whole forward+backward
+ * step measured 1.2-1.6x the default one (DESIGN.md §4 has the per-kernel times). */
+size_t dgr_det_scratch_bytes(uint64_t instances, int64_t records);
+int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom, const void *binning,
+                     uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii, const float *out_alpha,
+                     const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *det_scratch, uint64_t det_scratch_bytes,
+                     uint64_t instances, void *stream);
+int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom, const void *binning, uint64_t capacity_instances,
+                           int32_t staging, const void *image, const int32_t *radii, const DgrImageGrads *gin,
+                           const DgrGaussianGrads *gout, void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances,
+                           void *stream);
+int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, const void *binning,
+                                 uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii,
+                                 const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views, void *det_scratch,
+                                 uint64_t det_scratch_bytes, uint64_t instances, void *stream);
+
 /* Multi-GPU (view-sharded data parallelism, SURVEY.md §8e): all-reduce(sum) of the flat float32 gradient buffer over
  * NVLink with this library's own kernel.  The buffer lives in symmetric memory: peer_ptrs[w] (HOST array of `world` device
  * addresses) is rank w's copy mapped into this process; multicast_ptr, if non-zero, is the NVSwitch multicast address of
