@@ -67,6 +67,13 @@ class DgrViews(ctypes.Structure):
     ]
 
 
+class DgrRasterOptions(ctypes.Structure):
+    """Options of the *_ex calls (include/dgr_b200.h): flags = DGR_RASTER_* bits."""
+    _fields_ = [("flags", ctypes.c_uint32)]
+
+
+RASTER_ANTIALIAS = 1                 # DGR_RASTER_ANTIALIAS
+
 VIEWS_MAX = 64                       # DGR_VIEWS_MAX
 VIEWS_MAX_RECORDS = 2 ** 31 - 1      # DGR_VIEWS_MAX_RECORDS: V x P
 
@@ -86,6 +93,9 @@ EXPORTS = (
     "dgr_views_mixed_geom_bytes", "dgr_views_mixed_image_bytes", "dgr_views_mixed_forward_preprocess",
     "dgr_views_mixed_forward_render", "dgr_views_mixed_backward",
     "dgr_det_scratch_bytes", "dgr_backward_det", "dgr_views_backward_det", "dgr_views_mixed_backward_det",
+    "dgr_forward_preprocess_ex", "dgr_views_forward_preprocess_ex", "dgr_views_mixed_forward_preprocess_ex",
+    "dgr_backward_ex", "dgr_views_backward_ex", "dgr_views_mixed_backward_ex",
+    "dgr_backward_det_ex", "dgr_views_backward_det_ex", "dgr_views_mixed_backward_det_ex",
 )
 
 _lib = None
@@ -203,6 +213,13 @@ def load():
     lib.dgr_views_backward_det.argtypes = list(lib.dgr_views_backward.argtypes[:-1]) + [vp, u64, u64, vp]
     lib.dgr_views_mixed_backward_det.restype = ctypes.c_int
     lib.dgr_views_mixed_backward_det.argtypes = list(lib.dgr_views_mixed_backward.argtypes[:-1]) + [vp, u64, u64, vp]
+    # the *_ex calls: the counterpart's arguments + const DgrRasterOptions * (NULL = flags 0) before the stream
+    for name in ("dgr_forward_preprocess", "dgr_views_forward_preprocess", "dgr_views_mixed_forward_preprocess", "dgr_backward",
+                 "dgr_views_backward", "dgr_views_mixed_backward", "dgr_backward_det", "dgr_views_backward_det",
+                 "dgr_views_mixed_backward_det"):
+        ex = getattr(lib, name + "_ex")
+        ex.restype = ctypes.c_int
+        ex.argtypes = list(getattr(lib, name).argtypes[:-1]) + [ctypes.POINTER(DgrRasterOptions), vp]
     if lib.dgr_abi_version() != ABI_VERSION:
         raise RuntimeError("libdgr_b200.so ABI version mismatch")
     _lib = lib

@@ -44,7 +44,9 @@ def source_hash():
     return h.hexdigest()
 
 
-STEP_SOURCES = ("dgr_common.cuh", "dgr_preprocess.cuh", "dgr_binning.cuh", "dgr_render.cuh", "dgr_backward.cuh", "dgr_api.cu")
+STEP_SOURCES = ("dgr_common.cuh", "dgr_preprocess.cuh", "dgr_preprocess_fwd_body.cuh", "dgr_preprocess_views_fwd_body.cuh",
+                "dgr_binning.cuh", "dgr_render.cuh", "dgr_backward.cuh", "dgr_backward_body.cuh", "dgr_backward_views_body.cuh",
+                "dgr_api.cu")
 
 
 def step_kernel_hash():

@@ -161,9 +161,34 @@ PreFwdSmem pre_fwd_smem(const DgrGaussians *g, bool stageable, bool raw, int til
 }
 
 
+// ---- rasterization options (DgrRasterOptions) ----------------------------------------------------------------------------------
+// The forward's flags live in one byte of the image scratch's work block, past TileWork: the forward's memset zeroes it (flags 0
+// costs nothing) and an anti-aliased forward sets it; a backward with debug set compares it with its own flags.
+constexpr size_t kFlagsByte = 255;
+static_assert(sizeof(TileWork) <= kFlagsByte, "the flags byte must lie past TileWork (clear_costs_for_rerun zeroes up to its end)");
+static_assert(DGR_RASTER_ANTIALIAS < 256u, "the known flags must fit the flags byte");
+
+int raster_flags(const DgrRasterOptions *opt, uint32_t *flags) {
+    *flags = opt ? opt->flags : 0u;
+    if (*flags & ~DGR_RASTER_ANTIALIAS) return fail(-1, "DgrRasterOptions: unknown flag bits");
+    return 0;
+}
+int record_flags(char *image, const ImageLayout &IL, uint32_t flags, cudaStream_t st) {
+    if (flags) DGR_CUDA(cudaMemsetAsync(image + IL.off_work + kFlagsByte, (int)flags, 1, st));
+    return 0;
+}
+int check_forward_flags(const void *image, const ImageLayout &IL, uint32_t flags, int debug, cudaStream_t st) {
+    if (!debug) return 0;
+    unsigned char fwd = 0;
+    DGR_CUDA(cudaMemcpyAsync(&fwd, (const char *)image + IL.off_work + kFlagsByte, 1, cudaMemcpyDeviceToHost, st));
+    DGR_CUDA(cudaStreamSynchronize(st));
+    if (fwd != flags) return fail(-1, "backward: DgrRasterOptions.flags differ from those of the forward (antialiasing)");
+    return 0;
+}
+
 template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW>
 void launch_pre_fwd(const DgrSettings *s, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L, unsigned *tile_count,
-                    cudaStream_t st) {
+                    bool aa, cudaStream_t st) {
     const PreFwdSmem sm = pre_fwd_smem(g, HAS_SH && !HAS_COV, RAW, L.tiles, 0);
     auto launch = [&](auto kernel) {
         if (sm.bytes > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.bytes);
@@ -174,14 +199,19 @@ void launch_pre_fwd(const DgrSettings *s, const DgrGaussians *g, int *radii, cha
             tile_count, reinterpret_cast<unsigned *>(geom + L.off_runs), L.tiles, L.iters, (int)sm.stage_off);
     };
     if constexpr (HAS_SH && !HAS_COV) {
-        if (sm.staged) return launch(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>);
+        if (sm.staged) {
+            if (aa) launch(preprocess_fwd_aa_kernel<DEG, HAS_SH, HAS_COV, RAW, true>);
+            else launch(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>);
+            return;
+        }
     }
-    launch(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>);
+    if (aa) launch(preprocess_fwd_aa_kernel<DEG, HAS_SH, HAS_COV, RAW, false>);
+    else launch(preprocess_fwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>);
 }
 
 template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW>
 void launch_pre_bwd(const DgrSettings *s, const DgrGaussians *g, const int *radii, const unsigned *touched, const float *grad_rec,
-                    const DgrGaussianGrads *o, cudaStream_t st) {
+                    const DgrGaussianGrads *o, bool aa, cudaStream_t st) {
     const int nb = (g->P + kPreThreads - 1) / kPreThreads;
     PeerPush push;
     memset(&push, 0, sizeof(push));
@@ -189,26 +219,26 @@ void launch_pre_bwd(const DgrSettings *s, const DgrGaussians *g, const int *radi
         push.per = (int)o->push->gaussians_per_owner;
         for (int w = 0; w < o->push->world && w < kMaxPeers; w++) push.delta[w] = o->push->delta_floats[w];
     }
+    auto launch = [&](auto kernel, size_t smem, int wfl) {
+        if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        launch_k(kernel, dim3(nb), dim3(kPreThreads), smem, st, true,
+            g->P, g->M, s->image_height, s->image_width, s->tanfovx, s->tanfovy, s->scale_modifier, s->viewmatrix, s->projmatrix,
+            s->campos, g->means3D, g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, g->cov3D_precomp, radii, touched, grad_rec,
+            o->dL_dmeans3D, o->dL_dmeans2D, o->dL_dshs, o->dL_dcolors_precomp, o->dL_dopacities, o->dL_dscales, o->dL_drotations,
+            o->dL_dcov3D_precomp, o->dL_dshs_rest, o->xyz_gradient_accum, o->denom, o->max_radii2D, o->accumulate, push, wfl);
+    };
     if constexpr (HAS_SH && !HAS_COV) {
         // inputs staged by bulk TMA; the same per-warp slice of dynamic shared memory is the warp's output image afterwards
         const int wfl = max(stage_warp_floats(g->M), kStageFloats);
         const size_t smem = (size_t)(kPreThreads / 32) * wfl * 4;
         if (g_stage_bwd.load() && stage_inputs_ok(g, RAW) && smem + 1024 <= kMaxKernelSmem) {
-            if (smem > 48 * 1024)
-                cudaFuncSetAttribute(preprocess_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            launch_k(preprocess_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>, dim3(nb), dim3(kPreThreads), smem, st, true,
-                g->P, g->M, s->image_height, s->image_width, s->tanfovx, s->tanfovy, s->scale_modifier, s->viewmatrix, s->projmatrix,
-                s->campos, g->means3D, g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, g->cov3D_precomp, radii, touched, grad_rec,
-                o->dL_dmeans3D, o->dL_dmeans2D, o->dL_dshs, o->dL_dcolors_precomp, o->dL_dopacities, o->dL_dscales, o->dL_drotations,
-                o->dL_dcov3D_precomp, o->dL_dshs_rest, o->xyz_gradient_accum, o->denom, o->max_radii2D, o->accumulate, push, wfl);
+            if (aa) launch(preprocess_bwd_aa_kernel<DEG, HAS_SH, HAS_COV, RAW, true>, smem, wfl);
+            else launch(preprocess_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true>, smem, wfl);
             return;
         }
     }
-    launch_k(preprocess_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, dim3(nb), dim3(kPreThreads), 0, st, true,
-        g->P, g->M, s->image_height, s->image_width, s->tanfovx, s->tanfovy, s->scale_modifier, s->viewmatrix, s->projmatrix,
-        s->campos, g->means3D, g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, g->cov3D_precomp, radii, touched, grad_rec,
-        o->dL_dmeans3D, o->dL_dmeans2D, o->dL_dshs, o->dL_dcolors_precomp, o->dL_dopacities, o->dL_dscales, o->dL_drotations,
-        o->dL_dcov3D_precomp, o->dL_dshs_rest, o->xyz_gradient_accum, o->denom, o->max_radii2D, o->accumulate, push, 0);
+    if (aa) launch(preprocess_bwd_aa_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, 0, 0);
+    else launch(preprocess_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, 0, 0);
 }
 
 #define DGR_DISPATCH(FN, ...)                                                                              \
@@ -499,8 +529,8 @@ size_t dgr_geom_bytes(int32_t P, int32_t H, int32_t W) { return GeomLayout(P, H,
 size_t dgr_image_bytes(int32_t H, int32_t W) { return ImageLayout(H, W).total; }
 size_t dgr_binning_bytes(uint64_t cap, int32_t H, int32_t W) { (void)H; (void)W; return BinningLayout(cap).total; }
 
-int dgr_forward_preprocess(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
-    NvtxRange nvtx_("dgr_forward_preprocess");
+static int forward_preprocess(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, uint32_t flags,
+                              void *stream) {
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
     cudaStream_t st = (cudaStream_t)stream;
@@ -511,11 +541,26 @@ int dgr_forward_preprocess(const DgrSettings *s, const DgrGaussians *g, void *ge
     if ((size_t)L.tiles * 4 > kMaxTileSmem) return fail(-3, "image has more than 51200 tiles (16x16): not supported");
     // one memset: the work block + the per-tile instance totals the preprocess kernel adds into + the backward cost accumulators
     DGR_CUDA(cudaMemsetAsync(image + IL.off_work, 0, (IL.off_cost - IL.off_work) + (size_t)L.tiles * 8 * 4, st));
+    if (int e = record_flags(image, IL, flags, st)) return e;
+    const bool aa = flags & DGR_RASTER_ANTIALIAS;
     if (g->P > 0) {
         if (!radii) return fail(-1, "radii is NULL");
-        DGR_KERNEL("preprocess_fwd", st, s->debug, DGR_DISPATCH(launch_pre_fwd, s, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), st));
+        DGR_KERNEL("preprocess_fwd", st, s->debug, DGR_DISPATCH(launch_pre_fwd, s, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), aa, st));
     }
     return 0;
+}
+
+int dgr_forward_preprocess(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
+    NvtxRange nvtx_("dgr_forward_preprocess");
+    return forward_preprocess(s, g, geom_v, image_v, radii, 0u, stream);
+}
+
+int dgr_forward_preprocess_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii,
+                              const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_forward_preprocess_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    return forward_preprocess(s, g, geom_v, image_v, radii, flags, stream);
 }
 
 int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
@@ -613,7 +658,7 @@ static int flat_segs(int32_t n_seg, const int64_t *seg_off, const int32_t *seg_s
 // dgr_backward (det = NULL) and dgr_backward_det
 static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                            int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                           const DgrGaussianGrads *gout, const DetArgs *det, void *stream) {
+                           const DgrGaussianGrads *gout, const DetArgs *det, uint32_t flags, void *stream) {
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -631,6 +676,7 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
     GeomLayout GL(g->P, H, W);
     ImageLayout IL(H, W);
     BinningLayout BL(capacity);
+    if (int e = check_forward_flags(image, IL, flags, s->debug, st)) return e;
     const int tiles = IL.gx * IL.gy;
     float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
     // one memset: the work counter of the persistent backward render kernel + the per-Gaussian moment accumulators
@@ -685,7 +731,8 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
 #undef DGR_RENDER_BWD_L
 #undef DGR_RENDER_BWD
     }
-    DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, st));
+    const bool aa = flags & DGR_RASTER_ANTIALIAS;
+    DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, aa, st));
     return 0;
 }
 
@@ -694,7 +741,17 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
                  const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_backward");
     (void)out_alpha;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, stream);
+}
+
+int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
+                    int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                    const DgrGaussianGrads *gout, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_backward_ex");
+    (void)out_alpha;
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, stream);
 }
 
 size_t dgr_det_scratch_bytes(uint64_t instances, int64_t records) { return DetLayout(instances, records).total; }
@@ -705,7 +762,19 @@ int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom_v, 
     NvtxRange nvtx_("dgr_backward_det");
     (void)out_alpha;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, stream);
+}
+
+int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
+                        int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                        const DgrGaussianGrads *gout, void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances,
+                        const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_backward_det_ex");
+    (void)out_alpha;
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    const DetArgs det{det_scratch, det_scratch_bytes, instances};
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, stream);
 }
 
 }  // extern "C"
@@ -805,7 +874,7 @@ constexpr size_t kViewsFwdStaticSmem = (size_t)kMaxViews * (sizeof(FrameConsts) 
 
 template <int DEG, bool RAW>
 void launch_views_pre_fwd(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, int *radii, char *geom, const GeomLayout &L,
-                          unsigned *tile_count, cudaStream_t st) {
+                          unsigned *tile_count, bool aa, cudaStream_t st) {
     const PreFwdSmem sm = pre_fwd_smem(g, true, RAW, L.tiles, kViewsFwdStaticSmem);
     auto launch = [&](auto kernel) {
         if (sm.bytes + kViewsFwdStaticSmem > 48 * 1024)          // the cameras' static shared memory counts against the 48 KB
@@ -815,14 +884,20 @@ void launch_views_pre_fwd(const DgrViews *s, const ViewsBatch &b, const DgrGauss
                  g->scales, g->rotations, radii, reinterpret_cast<Rec *>(geom + L.off_rec), reinterpret_cast<unsigned *>(geom + L.off_touched),
                  tile_count, reinterpret_cast<unsigned *>(geom + L.off_runs), L.iters, (int)sm.stage_off);
     };
-    if (sm.staged) launch(preprocess_views_fwd_kernel<DEG, RAW, true>);
-    else launch(preprocess_views_fwd_kernel<DEG, RAW, false>);
+    if (aa) {
+        if (sm.staged) launch(preprocess_views_fwd_aa_kernel<DEG, RAW, true>);
+        else launch(preprocess_views_fwd_aa_kernel<DEG, RAW, false>);
+    } else {
+        if (sm.staged) launch(preprocess_views_fwd_kernel<DEG, RAW, true>);
+        else launch(preprocess_views_fwd_kernel<DEG, RAW, false>);
+    }
 }
 
 template <int DEG, bool RAW>
 void launch_views_pre_bwd(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, const int *radii, const unsigned *touched,
-                          const float *grad_rec, const DgrGaussianGrads *o, uint64_t stats_views, cudaStream_t st) {
-    launch_k(preprocess_views_bwd_kernel<DEG, RAW>, dim3((g->P + kPreThreads - 1) / kPreThreads), dim3(kPreThreads), 0, st, true,
+                          const float *grad_rec, const DgrGaussianGrads *o, uint64_t stats_views, bool aa, cudaStream_t st) {
+    launch_k(aa ? preprocess_views_bwd_aa_kernel<DEG, RAW> : preprocess_views_bwd_kernel<DEG, RAW>, dim3((g->P + kPreThreads - 1) / kPreThreads),
+             dim3(kPreThreads), 0, st, true,
              g->P, g->M, s->V, b.vt, s->scale_modifier, s->tanfov, s->viewmatrix, s->projmatrix, s->campos,
              g->means3D, g->shs, g->shs_rest, g->opacities, g->scales, g->rotations, radii, touched, grad_rec, o->dL_dmeans3D,
              o->dL_dmeans2D, o->dL_dshs, o->dL_dopacities, o->dL_dscales, o->dL_drotations, o->dL_dshs_rest, o->xyz_gradient_accum,
@@ -846,7 +921,8 @@ void launch_views_pre_bwd(const DgrViews *s, const ViewsBatch &b, const DgrGauss
     } while (0)
 
 // The three stages of a checked batch (s, g and the sizes in b).
-int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, void *stream) {
+int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, uint32_t flags,
+                     void *stream) {
     char *geom = (char *)geom_v, *image = (char *)image_v;
     if (!geom || !image) return fail(-1, "geom / image scratch is NULL");
     if (g->P > 0 && !radii) return fail(-1, "radii is NULL");
@@ -854,9 +930,11 @@ int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians 
     const GeomLayout L = GeomLayout::batch(g->P, b.tiles, s->V);
     const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
     DGR_CUDA(cudaMemsetAsync(image + IL.off_work, 0, (IL.off_cost - IL.off_work) + (size_t)L.tiles * 8 * 4, st));
+    if (int e = record_flags(image, IL, flags, st)) return e;
+    const bool aa = flags & DGR_RASTER_ANTIALIAS;
     if (g->P > 0)
         DGR_KERNEL("preprocess_views_fwd", st, s->debug,
-                   DGR_VIEWS_DISPATCH(launch_views_pre_fwd, s, b, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), st));
+                   DGR_VIEWS_DISPATCH(launch_views_pre_fwd, s, b, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), aa, st));
     return 0;
 }
 
@@ -920,7 +998,7 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
 
 int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                    int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views,
-                   const DetArgs *det, void *stream) {
+                   const DetArgs *det, uint32_t flags, void *stream) {
     if (det)
         if (int e = check_det(*det, gout, capacity, (long long)g->P * s->V)) return e;
     if (g->P == 0) return 0;
@@ -931,6 +1009,7 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
     const GeomLayout GL = GeomLayout::batch(g->P, b.tiles, s->V);
     const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
     BinningLayout BL(capacity);
+    if (int e = check_forward_flags(image, IL, flags, s->debug, st)) return e;
     const int tiles = b.tiles;
     float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
     DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * s->V * kGradRecFloats * 4, st));
@@ -965,9 +1044,10 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
         if (lazy) DGR_VIEWS_BWD(true); else DGR_VIEWS_BWD(false);
 #undef DGR_VIEWS_BWD
     }
+    const bool aa = flags & DGR_RASTER_ANTIALIAS;
     DGR_KERNEL("preprocess_views_bwd", st, s->debug,
                DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, b, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout,
-                                  stats_views, st));
+                                  stats_views, aa, st));
     return 0;
 }
 }  // namespace
@@ -982,7 +1062,17 @@ int dgr_views_forward_preprocess(const DgrViews *s, const DgrGaussians *g, void 
     NvtxRange nvtx_("dgr_views_forward_preprocess");
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
-    return views_preprocess(s, views_batch_uniform(s), g, geom_v, image_v, radii, stream);
+    return views_preprocess(s, views_batch_uniform(s), g, geom_v, image_v, radii, 0u, stream);
+}
+
+int dgr_views_forward_preprocess_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii,
+                                    const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_forward_preprocess_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_preprocess(s, views_batch_uniform(s), g, geom_v, image_v, radii, flags, stream);
 }
 
 int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
@@ -997,7 +1087,7 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
 
 static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                                const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
-                               const DetArgs *det, void *stream) {
+                               const DetArgs *det, uint32_t flags, void *stream) {
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1006,13 +1096,23 @@ static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *g
     if (gout->xyz_gradient_accum || gout->denom || gout->max_radii2D)
         return fail(-2, "views: the fused densification statistics are not supported by the batched call");
     if (int e = check_views_grads(gout)) return e;
-    return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, det, stream);
+    return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, det, flags,
+                          stream);
 }
 
 int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                        const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_views_backward");
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, stream);
+}
+
+int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                          const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
+                          const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_backward_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, stream);
 }
 
 int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1020,7 +1120,17 @@ int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_
                            void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, stream);
+}
+
+int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
+                              const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
+                              void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_backward_det_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    const DetArgs det{det_scratch, det_scratch_bytes, instances};
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, stream);
 }
 
 // ---- views of different sizes: image_hw = [V,2] (height, width) on the host ------------------------------------------------------
@@ -1043,7 +1153,17 @@ int dgr_views_mixed_forward_preprocess(const DgrViews *s, const int32_t *image_h
     NvtxRange nvtx_("dgr_views_mixed_forward_preprocess");
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
-    return views_preprocess(s, views_batch(s->V, image_hw, 2), g, geom_v, image_v, radii, stream);
+    return views_preprocess(s, views_batch(s->V, image_hw, 2), g, geom_v, image_v, radii, 0u, stream);
+}
+
+int dgr_views_mixed_forward_preprocess_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, void *image_v,
+                                          int32_t *radii, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_forward_preprocess_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    if (int e = check_views_mixed(s, image_hw)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_preprocess(s, views_batch(s->V, image_hw, 2), g, geom_v, image_v, radii, flags, stream);
 }
 
 int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, void *binning_v,
@@ -1058,7 +1178,7 @@ int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, c
 
 static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
                                 uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, void *stream) {
+                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, uint32_t flags, void *stream) {
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1072,14 +1192,25 @@ static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, cons
         return fail(-1, "views mixed: a densification statistic buffer is set but stats_views is 0");
     if (int e = check_views_grads(gout)) return e;
     return views_backward(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout,
-                          stats_views, det, stream);
+                          stats_views, det, flags, stream);
 }
 
 int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
                              uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
                              const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward");
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, 0u,
+                                stream);
+}
+
+int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
+                                uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                                const DgrGaussianGrads *gout, uint64_t stats_views, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_backward_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, flags,
+                                stream);
 }
 
 int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1088,7 +1219,19 @@ int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, con
                                  uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, 0u, stream);
+}
+
+int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
+                                    uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
+                                    const DgrGaussianGrads *gout, uint64_t stats_views, void *det_scratch, uint64_t det_scratch_bytes,
+                                    uint64_t instances, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_backward_det_ex");
+    uint32_t flags = 0;
+    if (int e = raster_flags(opt, &flags)) return e;
+    const DetArgs det{det_scratch, det_scratch_bytes, instances};
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, flags,
+                                stream);
 }
 
 }  // extern "C"

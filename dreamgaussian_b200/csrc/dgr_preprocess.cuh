@@ -220,6 +220,28 @@ __device__ __forceinline__ void project_geo(const FrameConsts &fc, const float3 
     g.cyy = g.T1[0] * ST1[0] + g.T1[1] * ST1[1] + g.T1[2] * ST1[2] + DGR_COV2D_LOWPASS;
 }
 
+// Anti-aliased mode (the 2D Mip filter of Mip-Splatting): the low-pass dilation keeps its conic, radius and tile rect, and the
+// opacity is scaled by comp = sqrt(max(DGR_AA_RATIO_FLOOR, det0 / det)) so that a Gaussian keeps its integrated weight at every
+// resolution.  det = the determinant of cov2D with the low-pass, det0 = without it, formed from the diagonal BEFORE the low-pass
+// (a0, c0 recomputed here from T and Sigma: subtracting 0.3 again would cost a sub-pixel Gaussian most of its float32 digits, and
+// keeping them in Geo would change the default kernels).
+struct AaCov { float a0, c0, ratio; };
+__device__ __forceinline__ AaCov aa_cov(const Geo &g, const float (&S6)[6], float det) {
+    const float Sg[9] = { S6[0], S6[1], S6[2], S6[1], S6[3], S6[4], S6[2], S6[4], S6[5] };
+    AaCov r;
+    r.a0 = 0.f; r.c0 = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        r.a0 += g.T0[k] * (Sg[3 * k] * g.T0[0] + Sg[3 * k + 1] * g.T0[1] + Sg[3 * k + 2] * g.T0[2]);
+        r.c0 += g.T1[k] * (Sg[3 * k] * g.T1[0] + Sg[3 * k + 1] * g.T1[1] + Sg[3 * k + 2] * g.T1[2]);
+    }
+    r.ratio = (r.a0 * r.c0 - g.cxy * g.cxy) / det;
+    return r;
+}
+__device__ __forceinline__ float aa_comp(const Geo &g, const float (&S6)[6], float det) {
+    return sqrtf(fmaxf(DGR_AA_RATIO_FLOOR, aa_cov(g, S6, det).ratio));
+}
+
 // ---- pieces shared by the single-view and the batched (dgr_views_*) per-Gaussian kernels --------------------------------
 // One Gaussian's inputs out of its warp's staging area (lane = the Gaussian's slot in the warp's run of 32).
 template <int DEG, bool RAW>
@@ -286,8 +308,9 @@ __device__ __forceinline__ void cov3d_from_inputs(float3 s_in, float4 q_in, floa
 
 // The camera-dependent part of the per-Gaussian forward for a Gaussian in front of the near plane: EWA cov2D, conic, radius,
 // pixel mean, SH -> RGB, opacity-aware pixel AABB, packed into the record.  Returns false (outputs untouched) when the Gaussian
-// is culled; otherwise the tiles it touches are those of for_each_touched_tile(r.q1.w, r.q2.w, ...).
-template <int DEG, bool HAS_SH, bool RAW>
+// is culled; otherwise the tiles it touches are those of for_each_touched_tile(r.q1.w, r.q2.w, ...).  AA: the record carries the
+// compensated opacity (aa_comp) and the opacity-aware pixel AABB is that of the compensated opacity.
+template <int DEG, bool HAS_SH, bool RAW, bool AA = false>
 __device__ __forceinline__ bool project_gaussian(const FrameConsts &fc, int H, int W, float tanfovx, float tanfovy, const float3 p,
                                                  const float (&S6)[6], float o_in, const float (&shc)[48], float dc0, float dc1, float dc2,
                                                  float pc0, float pc1, float pc2, Rec &r, int &radius_out, unsigned &clamp_flags) {
@@ -311,7 +334,8 @@ __device__ __forceinline__ bool project_gaussian(const FrameConsts &fc, int H, i
     const int rmaxy = min(gy, max(0, (int)((my + rad_f + (kTile - 1)) / kTile)));
     if (!(rmaxx > rminx && rmaxy > rminy)) return false;
     radius_out = (int)rad_f;
-    const float o = RAW ? act_sigmoid(o_in) : o_in;
+    float o = RAW ? act_sigmoid(o_in) : o_in;
+    if (AA) o *= aa_comp(geo, S6, det);
     // colour
     float cr, cg, cb;
     if (HAS_SH) {
@@ -377,195 +401,25 @@ __device__ __forceinline__ void publish_block_histogram(const unsigned *s_hist, 
     }
 }
 
+// Parameters of the single-view per-Gaussian forward kernels (preprocess_fwd_kernel, and preprocess_fwd_aa_kernel of the
+// anti-aliased mode); both compile the body in dgr_preprocess_fwd_body.cuh.
+#define DGR_PRE_FWD_PARAMS                                                                                                    \
+    int P, int M, int H, int W, float tanfovx, float tanfovy, float scale_modifier, const float *__restrict__ viewmatrix,      \
+        const float *__restrict__ projmatrix, const float *__restrict__ campos, const float *__restrict__ means3D,             \
+        const float *__restrict__ shs, const float *__restrict__ shs_rest, const float *__restrict__ colors_precomp,           \
+        const float *__restrict__ opacities, const float *__restrict__ scales, const float *__restrict__ rotations,            \
+        const float *__restrict__ cov3D_precomp, int *__restrict__ radii, Rec *__restrict__ rec, unsigned *__restrict__ touched_out, \
+        unsigned *__restrict__ tile_count, unsigned *__restrict__ run_matrix, int tiles, int gpb_iters, int stage_off
+
 template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW, bool STAGE = false>
-__global__ void __launch_bounds__(kPreThreads, 3)
-preprocess_fwd_kernel(int P, int M, int H, int W, float tanfovx, float tanfovy, float scale_modifier,
-                      const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix,
-                      const float *__restrict__ campos,
-                      const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ shs_rest,
-                      const float *__restrict__ colors_precomp, const float *__restrict__ opacities,
-                      const float *__restrict__ scales, const float *__restrict__ rotations,
-                      const float *__restrict__ cov3D_precomp,
-                      int *__restrict__ radii, Rec *__restrict__ rec, unsigned *__restrict__ touched_out,
-                      unsigned *__restrict__ tile_count, unsigned *__restrict__ run_matrix, int tiles, int gpb_iters, int stage_off) {
-    // Per-block tile histogram in shared memory (native integer smem atomics); at the end every touched tile's count is
-    // added to the per-tile totals with ONE global atomic per (block, tile) — not one per instance — and what the atomic
-    // returns (where this block's run starts inside the tile's range) goes into the block's row of the run matrix.
-    extern __shared__ __align__(128) unsigned s_hist[];
-    __shared__ FrameConsts fc;
-    __shared__ uint64_t s_stage_bar[kPreThreads / 32];
-    static_assert(!STAGE || (HAS_SH && !HAS_COV), "input staging: SH + scale / rotation inputs only");
-    pdl_trigger();                       // the tile scan may become resident now (it waits for this grid's completion)
-    // STAGE: this warp's inputs of the first block iteration are on their way before anything else happens
-    const int lane = threadIdx.x & 31;
-    float *wstage = STAGE ? reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(s_hist) + stage_off) + (threadIdx.x >> 5) * stage_warp_floats(M)
-                          : nullptr;
-    uint64_t *wbar = &s_stage_bar[threadIdx.x >> 5];
-    unsigned stage_phase = 0;
-    bool stage_inflight = false;         // warp-uniform: the copies of the NEXT block iteration have been started
-    if (STAGE) {
-        if (lane == 0) { mbar_init(wbar, 1); mbar_fence_init(); }
-        __syncwarp();
-        const int g0 = (int)(blockIdx.x * gpb_iters * kPreThreads + (threadIdx.x & ~31u));
-        stage_inflight = g0 + 32 <= P;
-        if (stage_inflight && lane == 0) stage_issue<RAW>(wstage, wbar, g0, M, means3D, scales, rotations, opacities, shs, shs_rest);
-    }
-    load_frame(fc, viewmatrix, projmatrix, HAS_SH ? campos : nullptr);
-    for (int t = threadIdx.x; t < tiles; t += kPreThreads) s_hist[t] = 0u;
-    __syncthreads();
-    for (int it = 0; it < gpb_iters; it++) {
-    const int g = (int)((blockIdx.x * gpb_iters + it) * kPreThreads + threadIdx.x);
-    unsigned touched = 0, clamp_flags = 0;
-    // every input of this Gaussian is requested before anything is computed (one memory round trip)
-    float3 p = make_float3(0.f, 0.f, 0.f);
-    float S6[6];
-    float3 s_in = make_float3(0.f, 0.f, 0.f);
-    float4 q_in = make_float4(1.f, 0.f, 0.f, 0.f);
-    float o_in = 0.f;
-    float shc[48], dc0 = 0.f, dc1 = 0.f, dc2 = 0.f, pc0 = 0.f, pc1 = 0.f, pc2 = 0.f;
-    const bool staged = STAGE && stage_inflight;                      // warp-uniform: all 32 Gaussians of this warp exist and are staged
-    if (staged) {
-        mbar_wait(wbar, stage_phase); stage_phase ^= 1u;
-        p = make_float3(wstage[kStgMean + 3 * lane], wstage[kStgMean + 3 * lane + 1], wstage[kStgMean + 3 * lane + 2]);
-        s_in = make_float3(wstage[kStgScale + 3 * lane], wstage[kStgScale + 3 * lane + 1], wstage[kStgScale + 3 * lane + 2]);
-        q_in = *reinterpret_cast<const float4 *>(wstage + kStgRot + 4 * lane);
-        o_in = wstage[kStgOp + lane];
-        if (RAW) {
-            dc0 = wstage[kStgSh + 3 * lane]; dc1 = wstage[kStgSh + 3 * lane + 1]; dc2 = wstage[kStgSh + 3 * lane + 2];
-            if (DEG > 0) lds_sh_row<DEG, 1>(wstage + kStgSh + 96 + lane * (M - 1) * 3, ((M - 1) & 3) == 0, shc);
-        } else lds_sh_row<DEG>(wstage + kStgSh + lane * M * 3, (M & 3) == 0, shc);
-    }
-    if (STAGE) {
-        __syncwarp();                    // every lane has its values in registers: the staging area is free for the next block iteration
-        stage_inflight = false;
-        if (it + 1 < gpb_iters) {
-            const int g0 = (int)((blockIdx.x * gpb_iters + it + 1) * kPreThreads + (threadIdx.x & ~31u));
-            stage_inflight = g0 + 32 <= P;
-            if (stage_inflight && lane == 0) stage_issue<RAW>(wstage, wbar, g0, M, means3D, scales, rotations, opacities, shs, shs_rest);
-        }
-    }
-    if (g < P) {
-        int radius_out = 0;
-        Rec r;
-        r.q0 = make_float4(0.f, 0.f, 0.f, 0.f); r.q1 = r.q0; r.q2 = r.q0;
-        if (!staged) {
-        p = make_float3(__ldg(means3D + 3 * (size_t)g), __ldg(means3D + 3 * (size_t)g + 1), __ldg(means3D + 3 * (size_t)g + 2));
-        if (HAS_COV) {
-#pragma unroll
-            for (int i = 0; i < 6; i++) S6[i] = __ldg(cov3D_precomp + 6 * (size_t)g + i);
-        } else {
-            s_in = make_float3(__ldg(scales + 3 * (size_t)g), __ldg(scales + 3 * (size_t)g + 1), __ldg(scales + 3 * (size_t)g + 2));
-            q_in = ldg_f4(rotations + 4 * (size_t)g);
-        }
-        o_in = __ldg(opacities + g);
-        if (HAS_SH) {
-            if (RAW) {          // _features_dc [P,1,3] + _features_rest [P,M-1,3]: no torch.cat copy
-                dc0 = __ldg(shs + 3 * (size_t)g); dc1 = __ldg(shs + 3 * (size_t)g + 1); dc2 = __ldg(shs + 3 * (size_t)g + 2);
-                if (DEG > 0) load_sh_row<DEG, 1>(shs_rest + (size_t)g * (M - 1) * 3, ((M - 1) & 3) == 0, shc);
-            } else load_sh_row<DEG>(shs + (size_t)g * M * 3, (M & 3) == 0, shc);
-        } else {
-            pc0 = __ldg(colors_precomp + 3 * (size_t)g); pc1 = __ldg(colors_precomp + 3 * (size_t)g + 1); pc2 = __ldg(colors_precomp + 3 * (size_t)g + 2);
-        }
-        }
-        const float tzc = p.x * fc.V[2] + p.y * fc.V[6] + p.z * fc.V[10] + fc.V[14];
-        if (tzc > DGR_NEAR_CULL_Z) {
-            if (!HAS_COV) {
-                float3 s = s_in;
-                if (RAW) s = make_float3(expf(s.x), expf(s.y), expf(s.z));
-                s = make_float3(scale_modifier * s.x, scale_modifier * s.y, scale_modifier * s.z);
-                float4 q = q_in;
-                if (RAW) { float inv; q = act_normalize(q, inv); }
-                float R[9]; quat_to_R(q, R);
-                cov3d_from_scale_rot(s, R, S6);
-            }
-            const float fx = (float)W / (2.f * tanfovx), fy = (float)H / (2.f * tanfovy);
-            Geo geo;
-            project_geo(fc, p, S6, fx, fy, DGR_FOV_CLAMP * tanfovx, DGR_FOV_CLAMP * tanfovy, geo);
-            const float det = geo.cxx * geo.cyy - geo.cxy * geo.cxy;
-            const float mid = 0.5f * (geo.cxx + geo.cyy);
-            const float lam = mid + sqrtf(fmaxf(DGR_EIG_FLOOR, mid * mid - det));
-            const float rad_f = ceilf(DGR_RADIUS_SIGMAS * sqrtf(lam));
-            const float mx = ((geo.ndcx + 1.f) * (float)W - 1.f) * 0.5f;
-            const float my = ((geo.ndcy + 1.f) * (float)H - 1.f) * 0.5f;
-            // det == 0 is the reference's cull; NaN / non-finite states (undefined upstream) are culled too.
-            const bool finite_ok = (det > 0.f) && (fabsf(mx) < 1e9f) && (fabsf(my) < 1e9f) && (rad_f < 1e9f);
-            if (finite_ok) {
-                const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-                // 3-sigma tile rect, truncation toward zero then clamp (reference rule)
-                const int rminx = min(gx, max(0, (int)((mx - rad_f) / kTile)));
-                const int rminy = min(gy, max(0, (int)((my - rad_f) / kTile)));
-                const int rmaxx = min(gx, max(0, (int)((mx + rad_f + (kTile - 1)) / kTile)));
-                const int rmaxy = min(gy, max(0, (int)((my + rad_f + (kTile - 1)) / kTile)));
-                if (rmaxx > rminx && rmaxy > rminy) {
-                    radius_out = (int)rad_f;
-                    const float o = RAW ? act_sigmoid(o_in) : o_in;
-                    // colour
-                    float cr, cg, cb;
-                    if (HAS_SH) {
-                        float dx = p.x - fc.cam[0], dy = p.y - fc.cam[1], dz = p.z - fc.cam[2];
-                        const float il = 1.f / sqrtf(dx * dx + dy * dy + dz * dz);
-                        dx *= il; dy *= il; dz *= il;
-                        float b[16]; sh_basis<DEG>(dx, dy, dz, b);
-                        constexpr int NB = (DEG + 1) * (DEG + 1);
-                        if (RAW) {
-                            cr = b[0] * dc0; cg = b[0] * dc1; cb = b[0] * dc2;
-#pragma unroll
-                            for (int k = 1; k < NB; k++) { cr += b[k] * shc[3 * (k - 1)]; cg += b[k] * shc[3 * (k - 1) + 1]; cb += b[k] * shc[3 * (k - 1) + 2]; }
-                        } else {
-                            cr = 0.f; cg = 0.f; cb = 0.f;
-#pragma unroll
-                            for (int k = 0; k < NB; k++) { cr += b[k] * shc[3 * k]; cg += b[k] * shc[3 * k + 1]; cb += b[k] * shc[3 * k + 2]; }
-                        }
-                        cr += DGR_SH_OFFSET; cg += DGR_SH_OFFSET; cb += DGR_SH_OFFSET;
-                        // channels clamped at 0 get no colour gradient: remembered in the top bits of `touched`
-                        clamp_flags = (cr < 0.f ? 1u : 0u) | (cg < 0.f ? 2u : 0u) | (cb < 0.f ? 4u : 0u);
-                        cr = fmaxf(cr, 0.f); cg = fmaxf(cg, 0.f); cb = fmaxf(cb, 0.f);
-                    } else {
-                        cr = pc0; cg = pc1; cb = pc2;
-                    }
-                    const float di = 1.f / det;
-                    const float cA = geo.cyy * di, cB = -geo.cxy * di, cC = geo.cxx * di;
-                    // opacity-aware pixel AABB: alpha >= 1/255  <=>  d^T conic d <= 2 ln(255 o)
-                    int bx0 = 1, bx1 = 0, by0 = 1, by1 = 0;
-                    const float o255 = o * 255.f;
-                    if (o255 > 1.f) {
-                        const float tau = 2.f * logf(o255);
-                        const float ex = sqrtf(tau * geo.cxx) * 1.0005f + 0.02f;
-                        const float ey = sqrtf(tau * geo.cyy) * 1.0005f + 0.02f;
-                        const float lim = 1e9f;
-                        bx0 = max(rminx * kTile, (int)ceilf(fmaxf(mx - ex, -lim)));
-                        by0 = max(rminy * kTile, (int)ceilf(fmaxf(my - ey, -lim)));
-                        bx1 = min(min(rmaxx * kTile, W) - 1, (int)floorf(fminf(mx + ex, lim)));
-                        by1 = min(min(rmaxy * kTile, H) - 1, (int)floorf(fminf(my + ey, lim)));
-                    }
-                    if (!(bx0 <= bx1 && by0 <= by1)) { bx0 = 1; bx1 = 0; by0 = 1; by1 = 0; }
-                    // conic stored as the coefficients of power*log2(e): -0.5 A log2e, -B log2e, -0.5 C log2e
-                    r.q0 = make_float4(mx, my, cA * (-0.5f * kLog2e), cB * (-kLog2e));
-                    r.q1 = make_float4(cC * (-0.5f * kLog2e), o, geo.t[2], __uint_as_float((unsigned)bx0 | ((unsigned)bx1 << 16)));
-                    r.q2 = make_float4(cr, cg, cb, __uint_as_float((unsigned)by0 | ((unsigned)by1 << 16)));
-                    // per-tile instance histogram of this block
-                    for_each_touched_tile(__float_as_uint(r.q1.w), __float_as_uint(r.q2.w), gx,
-                                          [&](int t) { atomicAdd(&s_hist[t], 1u); touched++; });
-                }
-            }
-        }
-        radii[g] = radius_out;
-        rec[g] = r;
-        touched_out[g] = touched | (clamp_flags << 29);     // tiles touched (29 bits) | SH clamp flags (3 bits)
-    }
-    }
-    __syncthreads();
-    unsigned *row = run_matrix + (size_t)blockIdx.x * tiles;
-    constexpr int kB = 12;                               // atomics in flight per thread (800 x 800: all 2500 tiles in ONE round trip)
-    for (int t0 = threadIdx.x; t0 < tiles; t0 += kPreThreads * kB) {
-        unsigned c[kB], got[kB];
-#pragma unroll
-        for (int j = 0; j < kB; j++) { const int t = t0 + j * kPreThreads; c[j] = t < tiles ? s_hist[t] : 0u; }
-#pragma unroll
-        for (int j = 0; j < kB; j++) got[j] = c[j] ? atomicAdd(tile_count + t0 + j * kPreThreads, c[j]) : 0u;
-#pragma unroll
-        for (int j = 0; j < kB; j++) { const int t = t0 + j * kPreThreads; if (t < tiles) row[t] = got[j]; }
-    }
+__global__ void __launch_bounds__(kPreThreads, 3) preprocess_fwd_kernel(DGR_PRE_FWD_PARAMS) {
+    constexpr bool AA = false;
+#include "dgr_preprocess_fwd_body.cuh"
+}
+template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW, bool STAGE = false>
+__global__ void __launch_bounds__(kPreThreads, 3) preprocess_fwd_aa_kernel(DGR_PRE_FWD_PARAMS) {
+    constexpr bool AA = true;
+#include "dgr_preprocess_fwd_body.cuh"
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -589,82 +443,24 @@ __device__ __forceinline__ void load_frames(FrameConsts *fcs, float2 *tan, int V
     for (int v = threadIdx.x; v < V; v += blockDim.x) tan[v] = make_float2(__ldg(tanfov + 2 * v), __ldg(tanfov + 2 * v + 1));
 }
 
+// Parameters of the batched per-Gaussian forward kernels; both compile the body in dgr_preprocess_views_fwd_body.cuh.
+#define DGR_VIEWS_FWD_PARAMS                                                                                                  \
+    int P, int M, int V, const __grid_constant__ ViewTable vt, float scale_modifier, const float *__restrict__ tanfov,          \
+        const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix, const float *__restrict__ campos,          \
+        const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ shs_rest,                  \
+        const float *__restrict__ opacities, const float *__restrict__ scales, const float *__restrict__ rotations,            \
+        int *__restrict__ radii, Rec *__restrict__ rec, unsigned *__restrict__ touched_out, unsigned *__restrict__ tile_count, \
+        unsigned *__restrict__ run_matrix, int gpb_iters, int stage_off
+
 template <int DEG, bool RAW, bool STAGE>
-__global__ void __launch_bounds__(kPreThreads, 3)
-preprocess_views_fwd_kernel(int P, int M, int V, const __grid_constant__ ViewTable vt, float scale_modifier, const float *__restrict__ tanfov,
-                            const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix, const float *__restrict__ campos,
-                            const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ shs_rest,
-                            const float *__restrict__ opacities, const float *__restrict__ scales, const float *__restrict__ rotations,
-                            int *__restrict__ radii, Rec *__restrict__ rec, unsigned *__restrict__ touched_out,
-                            unsigned *__restrict__ tile_count, unsigned *__restrict__ run_matrix, int gpb_iters, int stage_off) {
-    extern __shared__ __align__(128) unsigned s_hist[];                 // [tiles of the batch] histogram | STAGE: 8 warp staging areas
-    __shared__ FrameConsts s_fc[kMaxViews];
-    __shared__ float2 s_tan[kMaxViews];
-    __shared__ uint64_t s_stage_bar[kPreThreads / 32];
-    pdl_trigger();
-    const int lane = threadIdx.x & 31, tiles = vt.tile_off[V];
-    float *wstage = STAGE ? reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(s_hist) + stage_off) + (threadIdx.x >> 5) * stage_warp_floats(M)
-                          : nullptr;
-    uint64_t *wbar = &s_stage_bar[threadIdx.x >> 5];
-    unsigned stage_phase = 0;
-    bool stage_inflight = false;
-    if (STAGE) {
-        if (lane == 0) { mbar_init(wbar, 1); mbar_fence_init(); }
-        __syncwarp();
-        const int g0 = (int)(blockIdx.x * gpb_iters * kPreThreads + (threadIdx.x & ~31u));
-        stage_inflight = g0 + 32 <= P;
-        if (stage_inflight && lane == 0) stage_issue<RAW>(wstage, wbar, g0, M, means3D, scales, rotations, opacities, shs, shs_rest);
-    }
-    load_frames(s_fc, s_tan, V, tanfov, viewmatrix, projmatrix, campos);
-    for (int t = threadIdx.x; t < tiles; t += kPreThreads) s_hist[t] = 0u;
-    __syncthreads();
-    for (int it = 0; it < gpb_iters; it++) {
-        const int g = (int)((blockIdx.x * gpb_iters + it) * kPreThreads + threadIdx.x);
-        float3 p = make_float3(0.f, 0.f, 0.f), s_in = make_float3(0.f, 0.f, 0.f);
-        float4 q_in = make_float4(1.f, 0.f, 0.f, 0.f);
-        float S6[6], shc[48], o_in = 0.f, dc0 = 0.f, dc1 = 0.f, dc2 = 0.f, unused = 0.f;
-        const bool staged = STAGE && stage_inflight;
-        if (staged) {
-            mbar_wait(wbar, stage_phase); stage_phase ^= 1u;
-            lds_gaussian<DEG, RAW>(wstage, lane, M, p, s_in, q_in, o_in, dc0, dc1, dc2, shc);
-        }
-        if (STAGE) {
-            __syncwarp();
-            stage_inflight = false;
-            if (it + 1 < gpb_iters) {
-                const int g0 = (int)((blockIdx.x * gpb_iters + it + 1) * kPreThreads + (threadIdx.x & ~31u));
-                stage_inflight = g0 + 32 <= P;
-                if (stage_inflight && lane == 0) stage_issue<RAW>(wstage, wbar, g0, M, means3D, scales, rotations, opacities, shs, shs_rest);
-            }
-        }
-        if (g >= P) continue;
-        if (!staged)
-            ldg_gaussian<DEG, true, false, RAW>(g, M, means3D, shs, shs_rest, nullptr, opacities, scales, rotations, nullptr, p, S6, s_in, q_in,
-                                                o_in, dc0, dc1, dc2, shc, unused, unused, unused);
-        cov3d_from_inputs<RAW>(s_in, q_in, scale_modifier, S6);
-        for (int v = 0; v < V; v++) {
-            const FrameConsts &fc = s_fc[v];
-            unsigned touched = 0, clamp_flags = 0;
-            int radius_out = 0;
-            Rec r;
-            r.q0 = make_float4(0.f, 0.f, 0.f, 0.f); r.q1 = r.q0; r.q2 = r.q0;
-            const float tzc = p.x * fc.V[2] + p.y * fc.V[6] + p.z * fc.V[10] + fc.V[14];
-            if (tzc > DGR_NEAR_CULL_Z) {
-                const float2 tf = s_tan[v];
-                if (project_gaussian<DEG, true, RAW>(fc, vt.H[v], vt.W[v], tf.x, tf.y, p, S6, o_in, shc, dc0, dc1, dc2, 0.f, 0.f, 0.f, r,
-                                                     radius_out, clamp_flags)) {
-                    unsigned *vh = s_hist + vt.tile_off[v];
-                    for_each_touched_tile(__float_as_uint(r.q1.w), __float_as_uint(r.q2.w), vt.gx[v], [&](int t) { atomicAdd(&vh[t], 1u); touched++; });
-                }
-            }
-            const size_t rid = (size_t)v * P + g;
-            radii[rid] = radius_out;
-            rec[rid] = r;
-            touched_out[rid] = touched | (clamp_flags << 29);
-        }
-    }
-    __syncthreads();
-    publish_block_histogram(s_hist, tiles, tile_count, run_matrix);
+__global__ void __launch_bounds__(kPreThreads, 3) preprocess_views_fwd_kernel(DGR_VIEWS_FWD_PARAMS) {
+    constexpr bool AA = false;
+#include "dgr_preprocess_views_fwd_body.cuh"
+}
+template <int DEG, bool RAW, bool STAGE>
+__global__ void __launch_bounds__(kPreThreads, 3) preprocess_views_fwd_aa_kernel(DGR_VIEWS_FWD_PARAMS) {
+    constexpr bool AA = true;
+#include "dgr_preprocess_views_fwd_body.cuh"
 }
 
 __global__ void mark_visible_kernel(int P, const float *__restrict__ means3D, const float *__restrict__ V, unsigned char *present) {

@@ -52,6 +52,7 @@ struct State {                       // what one forward leaves behind for its b
     int64_t capacity = 0, n_inst = 0;
     int32_t staging = DGR_STAGING_SORTED;    // record staging the last stage-2 run chose (counts_host[3]): the backward's too
     int device = 0;
+    DgrRasterOptions opt{0u};                // the forward's options: its backward takes the same
 };
 
 // scratch of the deterministic backward (dgr_*_backward_det), taken when torch.use_deterministic_algorithms(True) is in effect
@@ -81,8 +82,9 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<State>>
 forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modifier, int64_t sh_degree, bool prefiltered, bool debug,
         const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const OptTensor &sh,
         const OptTensor &colors, const Tensor &opac, const OptTensor &scales, const OptTensor &rots, const OptTensor &cov3D,
-        const OptTensor &sh_rest, bool activations) {
+        const OptTensor &sh_rest, bool activations, bool antialiasing) {
     auto st = std::make_shared<State>();
+    st->opt.flags = antialiasing ? DGR_RASTER_ANTIALIAS : 0u;
     st->means3D = dev_f32(means3D, "means3D");
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     st->device = st->means3D.get_device();
@@ -128,7 +130,8 @@ forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modif
     st->geom = torch::empty({(int64_t)dgr_geom_bytes((int32_t)P, (int32_t)H, (int32_t)W)}, u8);
     st->image = torch::empty({(int64_t)dgr_image_bytes((int32_t)H, (int32_t)W)}, u8);
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
-    check(dgr_forward_preprocess(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), stream));
+    check(dgr_forward_preprocess_ex(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &st->opt,
+                                    stream));
     DgrImages out{color.data_ptr<float>(), depth.data_ptr<float>(), alpha.data_ptr<float>(), st->radii.data_ptr<int32_t>()};
     Hint hint{std::max<int64_t>(65536, 16 * P), true};
     const uint64_t key = hint_key(st->device, P, (int)H, (int)W);
@@ -199,13 +202,13 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
     if (at::globalContext().deterministicAlgorithms()) {
         Tensor det = det_scratch(st->n_inst, P, f32);
-        check(dgr_backward_det(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
-                               st->image.data_ptr(), st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, det.data_ptr(),
-                               (uint64_t)det.numel(), (uint64_t)st->n_inst, stream));
+        check(dgr_backward_det_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
+                                  st->image.data_ptr(), st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, det.data_ptr(),
+                                  (uint64_t)det.numel(), (uint64_t)st->n_inst, &st->opt, stream));
         return g;
     }
-    check(dgr_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
-                       st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, stream));
+    check(dgr_backward_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
+                          st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, &st->opt, stream));
     return g;
 }
 
@@ -221,6 +224,7 @@ struct ViewsState {
     int64_t capacity = 0, n_inst = 0;
     int32_t staging = DGR_STAGING_SORTED;
     int device = 0;
+    DgrRasterOptions opt{0u};
 };
 
 std::unordered_map<uint64_t, Hint> g_views_hints;       // keyed by (device, P, H, W, V), apart from the single-view hints
@@ -254,9 +258,11 @@ int64_t views_capacity_ceiling(int64_t V, int64_t H, int64_t W) {
 std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
 views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double scale_modifier, int64_t sh_degree, bool debug,
                    const Tensor &tanfov, const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D,
-                   const Tensor &sh, const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+                   const Tensor &sh, const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations,
+                   bool antialiasing) {
     auto st = std::make_shared<ViewsState>();
     st->hw = hw;
+    st->opt.flags = antialiasing ? DGR_RASTER_ANTIALIAS : 0u;
     const bool mixed = !hw.empty();
     st->means3D = dev_f32(means3D, "means3D");
     const c10::cuda::CUDAGuard guard(st->means3D.device());
@@ -307,12 +313,13 @@ views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double 
         const size_t gb = dgr_views_mixed_geom_bytes((int32_t)V, (int32_t)P, ihw), ib = dgr_views_mixed_image_bytes((int32_t)V, ihw);
         st->geom = torch::empty({(int64_t)std::max<size_t>(gb, 1)}, u8);
         st->image = torch::empty({(int64_t)std::max<size_t>(ib, 1)}, u8);
-        check(dgr_views_mixed_forward_preprocess(&st->s, ihw, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(),
-                                                 stream));
+        check(dgr_views_mixed_forward_preprocess_ex(&st->s, ihw, &st->g, st->geom.data_ptr(), st->image.data_ptr(),
+                                                    st->radii.data_ptr<int32_t>(), &st->opt, stream));
     } else {
         st->geom = torch::empty({(int64_t)dgr_views_geom_bytes((int32_t)V, (int32_t)P, (int32_t)H, (int32_t)W)}, u8);
         st->image = torch::empty({(int64_t)dgr_views_image_bytes((int32_t)V, (int32_t)H, (int32_t)W)}, u8);
-        check(dgr_views_forward_preprocess(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), stream));
+        check(dgr_views_forward_preprocess_ex(&st->s, &st->g, st->geom.data_ptr(), st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &st->opt,
+                                              stream));
     }
     DgrImages out{color.data_ptr<float>(), depth.data_ptr<float>(), alpha.data_ptr<float>(), st->radii.data_ptr<int32_t>()};
     const int64_t ceiling = views_capacity_ceiling(V, H, W);
@@ -364,21 +371,22 @@ views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double 
 std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
 views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov, const Tensor &bg,
               const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh, const Tensor &opac,
-              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations, bool antialiasing) {
     return views_forward_impl(H, W, {}, scale_modifier, sh_degree, debug, tanfov, bg, view, proj, campos, means3D, sh, opac, scales, rots,
-                              sh_rest, activations);
+                              sh_rest, activations, antialiasing);
 }
 
 // views of different sizes: image_hw = [V,2] (height, width); color [sum 3 H_v W_v], depth / alpha [sum H_v W_v] (flat)
 std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
 views_mixed_forward(const std::vector<int32_t> &image_hw, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov,
                     const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh,
-                    const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations) {
+                    const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations,
+                    bool antialiasing) {
     TORCH_CHECK_VALUE(!image_hw.empty() && image_hw.size() % 2 == 0, "image_hw must have dimensions (num_views, 2)");
     int64_t H = 0, W = 0;                                    // the capacity ceiling's bytes per instance do not depend on the size
     for (size_t i = 0; i < image_hw.size(); i += 2) { H = std::max<int64_t>(H, image_hw[i]); W = std::max<int64_t>(W, image_hw[i + 1]); }
     return views_forward_impl(H, W, image_hw, scale_modifier, sh_degree, debug, tanfov, bg, view, proj, campos, means3D, sh, opac, scales,
-                              rots, sh_rest, activations);
+                              rots, sh_rest, activations, antialiasing);
 }
 
 // grads: (means3D, means2D [V,P,3], shs | features_dc, opacities, scales, rotations, features_rest); the per-Gaussian ones summed over views.
@@ -409,20 +417,22 @@ std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, c
         Tensor det = det_scratch(st->n_inst, P * V, f32);
         const uint64_t n = (uint64_t)st->n_inst, bytes = (uint64_t)det.numel();
         if (!st->hw.empty())
-            check(dgr_views_mixed_backward_det(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
-                                               st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views,
-                                               det.data_ptr(), bytes, n, stream));
+            check(dgr_views_mixed_backward_det_ex(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(),
+                                                  (uint64_t)st->capacity, st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin,
+                                                  &gout, stats_views, det.data_ptr(), bytes, n, &st->opt, stream));
         else
-            check(dgr_views_backward_det(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
-                                         st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, det.data_ptr(), bytes, n, stream));
+            check(dgr_views_backward_det_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
+                                            st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, det.data_ptr(), bytes, n, &st->opt,
+                                            stream));
         return g;
     }
     if (!st->hw.empty())
-        check(dgr_views_mixed_backward(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
-                                       st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views, stream));
+        check(dgr_views_mixed_backward_ex(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
+                                          st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views, &st->opt,
+                                          stream));
     else
-        check(dgr_views_backward(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
-                                 st->radii.data_ptr<int32_t>(), &gin, &gout, stream));
+        check(dgr_views_backward_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
+                                    st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, &st->opt, stream));
     return g;
 }
 
@@ -437,17 +447,25 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     pybind11::class_<State, std::shared_ptr<State>>(m, "State")
         .def_readonly("capacity", &State::capacity)
         .def_readonly("num_rendered", &State::n_inst);
-    m.def("forward", &forward, "both forward stages through the C ABI (no arithmetic here)");
+    namespace py = pybind11;
+    m.def("forward", &forward, "both forward stages through the C ABI (no arithmetic here)", py::arg("H"), py::arg("W"), py::arg("tanfovx"),
+          py::arg("tanfovy"), py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("prefiltered"), py::arg("debug"), py::arg("bg"),
+          py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"), py::arg("sh"), py::arg("colors"), py::arg("opac"),
+          py::arg("scales"), py::arg("rots"), py::arg("cov3D"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("backward", &backward, "backward through the C ABI", pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"),
           pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"),
           pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0);
     pybind11::class_<ViewsState, std::shared_ptr<ViewsState>>(m, "ViewsState")
         .def_readonly("capacity", &ViewsState::capacity)
         .def_readonly("num_rendered", &ViewsState::n_inst);
-    m.def("views_forward", &views_forward, "both forward stages of the batched-camera call through the C ABI");
+    m.def("views_forward", &views_forward, "both forward stages of the batched-camera call through the C ABI", py::arg("H"), py::arg("W"),
+          py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("debug"), py::arg("tanfov"), py::arg("bg"), py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"),
+          py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("views_backward", &views_backward, "backward of the batched-camera call through the C ABI", pybind11::arg("state"),
           pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"));
-    m.def("views_mixed_forward", &views_mixed_forward, "both forward stages of the batched call with a size per view through the C ABI");
+    m.def("views_mixed_forward", &views_mixed_forward, "both forward stages of the batched call with a size per view through the C ABI",
+          py::arg("image_hw"), py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("debug"), py::arg("tanfov"), py::arg("bg"), py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"),
+          py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("views_mixed_backward", &views_backward_impl, "backward of the batched call with a size per view through the C ABI",
           pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"),
           pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"), pybind11::arg("denom"), pybind11::arg("max_radii2D"),

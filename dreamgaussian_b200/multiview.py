@@ -164,8 +164,9 @@ class ViewShardedRasterizer:
         self.grads.data.zero_()
 
     def render_views(self, params: dict, settings: Sequence[_r.GaussianRasterizationSettings],
-                     upstream: Sequence[tuple], keep_images: bool = False):
-        """upstream[i] = (dL_dcolor [3,H,W] or None, dL_ddepth or None, dL_dalpha or None) for local view i."""
+                     upstream: Sequence[tuple], keep_images: bool = False, antialiasing: bool = False):
+        """upstream[i] = (dL_dcolor [3,H,W] or None, dL_ddepth or None, dL_dalpha or None) for local view i.  antialiasing: as
+        GaussianRasterizer."""
         g = self.grads.views
         images = []
         if len(settings) == 0:
@@ -176,7 +177,8 @@ class ViewShardedRasterizer:
         self._pushed = False
         for i, (rs, up) in enumerate(zip(settings, upstream)):
             color, radii, depth, alpha, state = _r.forward_impl(
-                rs, params["means3D"], params["shs"], None, params["opacities"], params["scales"], params["rotations"], None)
+                rs, params["means3D"], params["shs"], None, params["opacities"], params["scales"], params["rotations"], None,
+                antialiasing=antialiasing)
             # the backward of the LAST local view also delivers the rows other ranks own (local sum of all this rank's views)
             # to their owners' staging areas: the reduce-scatter half of the all-reduce rides on that kernel
             # (not under torch.use_deterministic_algorithms: the deterministic backward takes no push, so the rows travel by

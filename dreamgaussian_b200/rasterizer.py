@@ -165,15 +165,22 @@ def _stream_ptr(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _raster_opts(antialiasing):
+    """The DgrRasterOptions argument of the *_ex calls."""
+    return ctypes.byref(_lib.DgrRasterOptions(_lib.RASTER_ANTIALIAS if antialiasing else 0))
+
+
 class ForwardState:
     """Everything one forward leaves behind for its backward (upstream: ctx + geom/binning/img buffers)."""
     __slots__ = ("rs", "frame", "num_rendered", "capacity", "staging", "geom", "binning", "image", "radii", "alpha", "tensors",
-                 "fast", "stats_applied")
+                 "fast", "stats_applied", "antialiasing")
 
 
-def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, sh_rest=None, activations=False):
+def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, sh_rest=None, activations=False,
+                 antialiasing=False):
     """Runs both forward stages through the C ABI. Inputs are validated CUDA float32 tensors (or None).
-    Returns (color, radii, depth, alpha, ForwardState).
+    Returns (color, radii, depth, alpha, ForwardState).  antialiasing: the 2D Mip filter with opacity compensation
+    (DGR_RASTER_ANTIALIAS, include/dgr_b200.h); the state remembers it for the backward.
 
     No host round trip sits between the kernels: the instance buffer is sized from a per-shape capacity hint, every
     kernel of the forward is enqueued, and only then does the host wait for the (early) instance-count event.  If the
@@ -182,9 +189,10 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
         color, radii, depth, alpha, cst = _FAST.forward(
             int(rs.image_height), int(rs.image_width), float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier), int(rs.sh_degree),
             bool(rs.prefiltered), bool(rs.debug), rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, means3D, sh, colors_precomp, opacities,
-            scales, rotations, cov3D, sh_rest, bool(activations))
+            scales, rotations, cov3D, sh_rest, bool(activations), bool(antialiasing))
         state = ForwardState()
         state.fast, state.rs, state.num_rendered, state.capacity = cst, rs, cst.num_rendered, cst.capacity
+        state.antialiasing = bool(antialiasing)
         state.radii, state.alpha = radii, None
         state.tensors = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, sh_rest)
         return color, radii, depth, alpha, state
@@ -202,8 +210,8 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
         image = torch.empty((lib.dgr_image_bytes(H, W),), **u8)
         n_host, event = _host_sync_objects(dev)
         st = _stream_ptr(dev)
-        _lib.check(lib.dgr_forward_preprocess(ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(geom), _ptr(image),
-                                              _ptr(radii), st))
+        _lib.check(lib.dgr_forward_preprocess_ex(ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(geom), _ptr(image),
+                                                 _ptr(radii), _raster_opts(antialiasing), st))
         out = _lib.DgrImages(_ptr(color), _ptr(depth), _ptr(alpha), _ptr(radii))
         key = (dev.index, P, H, W)
         cap, big = _CAPACITY_HINT.get(key, (max(65536, 16 * P), True))
@@ -222,7 +230,7 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
             rerun = 2                                   # DGR_FLAG_RERUN
         _CAPACITY_HINT[key] = (max(int(n_inst * 1.25) + 4096, 65536), n_big > 0)
     state = ForwardState()
-    state.fast = None
+    state.fast, state.antialiasing = None, bool(antialiasing)
     state.rs, state.frame, state.num_rendered, state.capacity = rs, fr, n_inst, cap
     state.staging = int(n_host[3])                  # record staging of the last stage-2 run: its backward must use the same
     # alpha is a differentiable OUTPUT: storing it here would close the cycle state -> alpha -> grad_fn -> ctx -> state and leave
@@ -274,9 +282,10 @@ def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2
                 ctypes.byref(gin), ctypes.byref(gout))
         if torch.are_deterministic_algorithms_enabled():
             det = _det_scratch(lib, state.num_rendered, fr.P, dev)
-            _lib.check(lib.dgr_backward_det(*args, *_det_args(det, state.num_rendered), _stream_ptr(dev)))
+            _lib.check(lib.dgr_backward_det_ex(*args, *_det_args(det, state.num_rendered), _raster_opts(state.antialiasing),
+                                               _stream_ptr(dev)))
         else:
-            _lib.check(lib.dgr_backward(*args, _stream_ptr(dev)))
+            _lib.check(lib.dgr_backward_ex(*args, _raster_opts(state.antialiasing), _stream_ptr(dev)))
 
 
 def _det_scratch(lib, instances, records, dev):
@@ -291,13 +300,14 @@ def _det_args(det, instances):
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                antialiasing=False):
         means3D = _dev_f32(means3D, "means3D")
         opacities = _dev_f32(opacities, "opacities")
         sh, colors_precomp = _opt(sh, "shs"), _opt(colors_precomp, "colors_precomp")
         scales, rotations, cov3D = _opt(scales, "scales"), _opt(rotations, "rotations"), _opt(cov3Ds_precomp, "cov3D_precomp")
         color, radii, depth, alpha, state = forward_impl(raster_settings, means3D, sh, colors_precomp, opacities, scales,
-                                                         rotations, cov3D)
+                                                         rotations, cov3D, antialiasing=antialiasing)
         ctx.state = state
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -307,7 +317,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         state = ctx.state
         if state.fast is not None:
             g = _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], None, None, None)      # undefined -> None
-            return g[0], g[1], g[2], g[3], g[4], g[5], g[6], g[7], None
+            return g[0], g[1], g[2], g[3], g[4], g[5], g[6], g[7], None, None
         means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, _ = state.tensors
         dev = means3D.device
         P, M = state.frame.P, state.frame.M
@@ -325,20 +335,24 @@ class _RasterizeGaussians(torch.autograd.Function):
         d_cov = torch.empty((P, 6), **f32) if cov3D is not None else None
         backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov)
         # ctx.state stays: a retain_graph backward runs again from the same buffers (they go away with the graph node)
-        return d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, None
+        return d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, None, None
 
 
-def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                        antialiasing=False):
+    """antialiasing=True: the 2D Mip filter with opacity compensation (Mip-Splatting), DGR_RASTER_ANTIALIAS of include/dgr_b200.h."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                     raster_settings)
+                                     raster_settings, bool(antialiasing))
 
 
 class GaussianRasterizer(nn.Module):
-    """Constructed per render call by the reference (gs_renderer.py:760): construction is trivial."""
+    """Constructed per render call by the reference (gs_renderer.py:760): construction is trivial.  antialiasing=True renders
+    with the 2D Mip filter and opacity compensation (include/dgr_b200.h, DGR_RASTER_ANTIALIAS); the settings keep their 12 fields."""
 
-    def __init__(self, raster_settings: GaussianRasterizationSettings):
+    def __init__(self, raster_settings: GaussianRasterizationSettings, antialiasing: bool = False):
         super().__init__()
         self.raster_settings = raster_settings
+        self.antialiasing = bool(antialiasing)
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -358,7 +372,7 @@ class GaussianRasterizer(nn.Module):
                 ((scales is not None or rotations is not None) and cov3D_precomp is not None):
             raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   self.raster_settings)
+                                   self.raster_settings, self.antialiasing)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -470,15 +484,16 @@ class _Views:
 class ViewsState:
     """Everything one batched forward leaves behind for its backward."""
     __slots__ = ("views", "capacity", "staging", "num_rendered", "geom", "binning", "image", "radii", "tensors", "fast", "mixed",
-                 "stats_applied")
+                 "stats_applied", "antialiasing")
 
 
-def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False, mixed=False):
+def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False, mixed=False,
+                       antialiasing=False):
     """Both forward stages of the batched call through the C ABI; inputs are validated CUDA float32 tensors.
     Returns (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W], ViewsState).  Same speculative-capacity
     protocol as forward_impl, with hints keyed by (device, P, H, W, V); the compiled host layer when it is loaded.
     mixed=True: every camera has its own image size (dgr_views_mixed_*); color [sum 3 H_v W_v], depth / alpha [sum H_v W_v]
-    are flat, view v's blocks one after the other, and the hints are keyed by (device, P, the sizes)."""
+    are flat, view v's blocks one after the other, and the hints are keyed by (device, P, the sizes).  antialiasing: as forward_impl."""
     lib = _lib.load()
     dev = means3D.device
     if _FAST is not None:
@@ -489,15 +504,15 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
             hw = [int(x) for s in settings_list for x in (s.image_height, s.image_width)]
             color, radii, depth, alpha, cst = _FAST.views_mixed_forward(
                 hw, float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams, means3D, sh, opacities, scales, rotations, sh_rest,
-                bool(activations))
+                bool(activations), bool(antialiasing))
         else:
             color, radii, depth, alpha, cst = _FAST.views_forward(
                 int(s0.image_height), int(s0.image_width), float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams,
-                means3D, sh, opacities, scales, rotations, sh_rest, bool(activations))
+                means3D, sh, opacities, scales, rotations, sh_rest, bool(activations), bool(antialiasing))
         state = ViewsState()
         state.fast, state.capacity, state.num_rendered, state.radii = cst, cst.capacity, cst.num_rendered, radii
         state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
-        state.mixed = mixed
+        state.mixed, state.antialiasing = mixed, bool(antialiasing)
         return color, radii, depth, alpha, state
     with torch.cuda.device(dev):
         vw = _Views(settings_list, means3D, sh, opacities, scales, rotations, sh_rest, activations, mixed=mixed)
@@ -515,14 +530,14 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
         if mixed:
             geom = torch.empty((max(1, lib.dgr_views_mixed_geom_bytes(V, P, vw.hw)),), **u8)
             image = torch.empty((max(1, lib.dgr_views_mixed_image_bytes(V, vw.hw)),), **u8)
-            _lib.check(lib.dgr_views_mixed_forward_preprocess(ctypes.byref(vw.settings), vw.hw, ctypes.byref(vw.gaussians), _ptr(geom),
-                                                              _ptr(image), _ptr(radii), st))
+            _lib.check(lib.dgr_views_mixed_forward_preprocess_ex(ctypes.byref(vw.settings), vw.hw, ctypes.byref(vw.gaussians), _ptr(geom),
+                                                                 _ptr(image), _ptr(radii), _raster_opts(antialiasing), st))
             key = ("views_mixed", dev.index, P, vw.sizes)
         else:
             geom = torch.empty((lib.dgr_views_geom_bytes(V, P, H, W),), **u8)
             image = torch.empty((lib.dgr_views_image_bytes(V, H, W),), **u8)
-            _lib.check(lib.dgr_views_forward_preprocess(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(image),
-                                                        _ptr(radii), st))
+            _lib.check(lib.dgr_views_forward_preprocess_ex(ctypes.byref(vw.settings), ctypes.byref(vw.gaussians), _ptr(geom), _ptr(image),
+                                                           _ptr(radii), _raster_opts(antialiasing), st))
             key = ("views", dev.index, P, H, W, V)
         out = _lib.DgrImages(_ptr(color), _ptr(depth), _ptr(alpha), _ptr(radii))
         ceiling = _views_capacity_ceiling(lib, dev, V, H, W)
@@ -547,7 +562,7 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
             rerun = 2                                   # DGR_FLAG_RERUN
         _CAPACITY_HINT[key] = (min(max(int(n_inst * 1.25) + 4096, 65536), _MAX_CAPACITY), n_big > 0)
     state = ViewsState()
-    state.fast, state.mixed = None, mixed
+    state.fast, state.mixed, state.antialiasing = None, mixed, bool(antialiasing)
     state.views, state.capacity, state.staging, state.num_rendered = vw, cap, int(n_host[3]), n_inst
     state.geom, state.binning, state.image, state.radii = geom, binning, image, radii
     state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
@@ -577,18 +592,21 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
                                      *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), None)
         common = (ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning), ctypes.c_uint64(state.capacity), state.staging,
                   _ptr(state.image), _ptr(state.radii), ctypes.byref(gin), ctypes.byref(gout))
+        opts = _raster_opts(state.antialiasing)
         if torch.are_deterministic_algorithms_enabled():
             det = _det_scratch(lib, state.num_rendered, vw.P * vw.V, dev)
             if state.mixed:
-                _lib.check(lib.dgr_views_mixed_backward_det(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views),
-                                                            *_det_args(det, state.num_rendered), _stream_ptr(dev)))
+                _lib.check(lib.dgr_views_mixed_backward_det_ex(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views),
+                                                               *_det_args(det, state.num_rendered), opts, _stream_ptr(dev)))
             else:
-                _lib.check(lib.dgr_views_backward_det(ctypes.byref(vw.settings), *common, *_det_args(det, state.num_rendered), _stream_ptr(dev)))
+                _lib.check(lib.dgr_views_backward_det_ex(ctypes.byref(vw.settings), *common, *_det_args(det, state.num_rendered), opts,
+                                                         _stream_ptr(dev)))
             return
         if state.mixed:
-            _lib.check(lib.dgr_views_mixed_backward(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views), _stream_ptr(dev)))
+            _lib.check(lib.dgr_views_mixed_backward_ex(ctypes.byref(vw.settings), vw.hw, *common, ctypes.c_uint64(stats_views), opts,
+                                                       _stream_ptr(dev)))
         else:
-            _lib.check(lib.dgr_views_backward(ctypes.byref(vw.settings), *common, _stream_ptr(dev)))
+            _lib.check(lib.dgr_views_backward_ex(ctypes.byref(vw.settings), *common, opts, _stream_ptr(dev)))
 
 
 def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, stats_views=0):
@@ -620,10 +638,11 @@ def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, sta
 
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False):
         means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
         sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
-        color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations)
+        color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
+                                                               antialiasing=antialiasing)
         ctx.state = state
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -632,32 +651,33 @@ class _RasterizeViews(torch.autograd.Function):
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
         d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=False)
         # ctx.state stays: a retain_graph backward runs again from the same buffers.  means2D may be None (no per-view gradient wanted)
-        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None
+        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None
 
 
-def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rotations):
+def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False):
     """Renders ONE cloud from every camera of `settings_list` (GaussianRasterizationSettings, at most 64, all with the same
     image_height / image_width / sh_degree / scale_modifier) in one batched forward, and one batched backward.
     Returns (color [V,3,H,W], radii int32 [V,P], depth [V,1,H,W], alpha [V,1,H,W]); view v equals what GaussianRasterizer
     returns for camera v.  The gradients of means3D / shs / opacities / scales / rotations are summed over the views;
     means2D is [V,P,3] (e.g. zeros with requires_grad) or None: its gradient is per view, for densification.  SH colours and
-    scale / rotation inputs only; no CPU path."""
+    scale / rotation inputs only; no CPU path.  antialiasing: as GaussianRasterizer."""
     settings_list = _check_views_settings(settings_list)
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
-    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list)
+    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list, bool(antialiasing))
 
 
 class GaussianViewsRasterizer(nn.Module):
     """`GaussianRasterizer` for a batch of same-size cameras: forward(means3D, means2D, opacities, shs, scales, rotations)
     -> (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]), see rasterize_views."""
 
-    def __init__(self, settings_list):
+    def __init__(self, settings_list, antialiasing=False):
         super().__init__()
         self.settings_list = _check_views_settings(settings_list)
+        self.antialiasing = bool(antialiasing)
 
     def forward(self, means3D, means2D, opacities, shs, scales, rotations):
-        return rasterize_views(self.settings_list, means3D, means2D, opacities, shs, scales, rotations)
+        return rasterize_views(self.settings_list, means3D, means2D, opacities, shs, scales, rotations, self.antialiasing)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -678,10 +698,11 @@ def split_views(settings_list, color, depth, alpha):
 
 class _RasterizeViewsMixed(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False):
         means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
         sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
-        color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, mixed=True)
+        color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, mixed=True,
+                                                               antialiasing=antialiasing)
         ctx.state = state
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -689,17 +710,19 @@ class _RasterizeViewsMixed(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
         d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=False)
-        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None
+        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None
 
 
-def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scales, rotations):
+def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False):
     """rasterize_views for cameras of DIFFERENT image sizes (at most 64, one sh_degree / scale_modifier): one batched forward
     and one batched backward.  Returns (colors, radii, depths, alphas): colors a list of [3,H_v,W_v], depths / alphas lists of
     [1,H_v,W_v] (views of one flat tensor each), radii int32 [V,P]; view v equals what GaussianRasterizer returns for camera v.
-    The gradients of means3D / shs / opacities / scales / rotations are summed over the views; means2D is [V,P,3] or None."""
+    The gradients of means3D / shs / opacities / scales / rotations are summed over the views; means2D is [V,P,3] or None.
+    antialiasing: as GaussianRasterizer."""
     settings_list = _check_views_mixed_settings(settings_list)
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
-    color, radii, depth, alpha = _RasterizeViewsMixed.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list)
+    color, radii, depth, alpha = _RasterizeViewsMixed.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list,
+                                                            bool(antialiasing))
     colors, depths, alphas = split_views(settings_list, color, depth, alpha)
     return colors, radii, depths, alphas

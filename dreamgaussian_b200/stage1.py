@@ -303,6 +303,7 @@ class Stage1Config(NamedTuple):
     opacity_reset_interval: int = 700
     densify_grad_threshold: float = 0.01
     seed: int = 0
+    antialiasing: bool = False          # every render with the 2D Mip filter and opacity compensation (GaussianRasterizer's switch)
 
 
 class GuidanceStub:
@@ -375,11 +376,11 @@ class Stage1Trainer:
         g = self.gaussians
         means2D = torch.zeros_like(g._xyz, requires_grad=True)
         if self.fused:
-            color, radii, depth, alpha = FusedGaussianRasterizer(rs)(g._xyz, g._features_dc, g._features_rest, g._opacity, g._scaling,
+            color, radii, depth, alpha = FusedGaussianRasterizer(rs, self.cfg.antialiasing)(g._xyz, g._features_dc, g._features_rest, g._opacity, g._scaling,
                                                                      g._rotation, means2D=means2D, stats=g.stats if track_stats else None)
         else:
             from .rasterizer import GaussianRasterizer
-            color, radii, depth, alpha = GaussianRasterizer(rs)(
+            color, radii, depth, alpha = GaussianRasterizer(rs, self.cfg.antialiasing)(
                 means3D=g._xyz, means2D=means2D, shs=torch.cat((g._features_dc, g._features_rest), dim=1),
                 opacities=torch.sigmoid(g._opacity), scales=torch.exp(g._scaling), rotations=torch.nn.functional.normalize(g._rotation))
         return {"image": color.clamp(0, 1), "alpha": alpha, "viewspace_points": means2D, "visibility_filter": radii > 0, "radii": radii}
@@ -429,7 +430,7 @@ class Stage1Trainer:
         novel, ver, hor = self._novel_camera(step_ratio)
         colors, radii, depths, alphas = rasterize_views_mixed_raw(
             [self.fixed_cam, novel], g._xyz, None, g._features_dc, g._features_rest, g._opacity, g._scaling, g._rotation,
-            stats=g.stats if densify_window else None, stats_views=(1,) if densify_window else ())
+            stats=g.stats if densify_window else None, stats_views=(1,) if densify_window else (), antialiasing=cfg.antialiasing)
         loss = 10000 * step_ratio * torch.nn.functional.mse_loss(colors[0].clamp(0, 1).unsqueeze(0), self.input_img)
         loss = loss + 1000 * step_ratio * torch.nn.functional.mse_loss(alphas[0].unsqueeze(0), self.input_mask)
         return loss + cfg.lambda_zero123 * self.guidance.train_step(colors[1].clamp(0, 1).unsqueeze(0), [ver], [hor], [0], step_ratio=step_ratio,

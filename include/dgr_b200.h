@@ -286,6 +286,59 @@ int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, con
                                  const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views, void *det_scratch,
                                  uint64_t det_scratch_bytes, uint64_t instances, void *stream);
 
+/* == Rasterization options: anti-aliased rendering (the 2D Mip filter with opacity compensation) ==
+ * The *_ex calls take the arguments of their counterparts plus `opt` (NULL = flags 0); with flags 0 they compute exactly what the
+ * counterpart computes.  DGR_RASTER_ANTIALIAS: per Gaussian and view, with (a0, b, c0) the 2D covariance in pixels before the
+ * low-pass and (a, b, c) = (a0 + 0.3, b, c0 + 0.3) after it, the opacity o (raw parameters: sigmoid first) is replaced by
+ *   o_eff = o sqrt(max(DGR_AA_RATIO_FLOOR, (a0 c0 - b^2) / (a c - b^2)))          (Mip-Splatting, Yu et al., CVPR 2024)
+ * so a Gaussian smaller than a pixel keeps its integrated weight instead of being dilated and brightened at a low resolution:
+ * its image changes little across resolutions and scale_modifier.  Radii, the tile rectangle and the conic are those of the
+ * default mode; alpha = min(0.99, o_eff G) with the other compositing rules unchanged; the opacity-aware pixel box follows o_eff,
+ * so there are at most as many tile instances as in the default mode.  Gradients are the exact chain rule, with the factor
+ * differentiated through the determinant ratio into the 2D covariance (no gradient where the floor is active).
+ * Limit: a0 c0 - b^2 is formed in float32 from the covariance entries (as upstream diff-gaussian-rasterization forms it); its
+ * relative error is about 3e-8 r^2 for a footprint of aspect ratio r, so needles beyond ~100:1 get a compensation with a float32
+ * error of 1e-4 or more, and for a needle far thinner than a pixel and hundreds of pixels long it is rounding noise.
+ * The forward's flags are recorded in its `image` scratch; its backward must be given the same flags.  With debug set
+ * (DgrSettings / DgrViews) the backward compares them (one host synchronisation) and refuses a mismatch; without debug a mismatch
+ * is not detected and gives wrong gradients.  Refused before any device work: unknown flag bits, and everything the counterpart
+ * refuses.  Each call accepts everything its counterpart accepts (DgrPeerPush included where the counterpart takes it); the
+ * stage-2 render calls need no variant.
+ * Cost: only the per-Gaussian forward and backward kernels differ (their *_aa_kernel variants: a few dozen FLOPs and a square
+ * root per Gaussian and view); the binning, sort and render kernels are those of the default mode (DESIGN.md §4 has the times). */
+#define DGR_RASTER_ANTIALIAS 1u
+typedef struct DgrRasterOptions {
+    uint32_t flags;          /* DGR_RASTER_* bits */
+} DgrRasterOptions;
+int dgr_forward_preprocess_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii,
+                              const DgrRasterOptions *opt, void *stream);
+int dgr_views_forward_preprocess_ex(const DgrViews *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii,
+                                    const DgrRasterOptions *opt, void *stream);
+int dgr_views_mixed_forward_preprocess_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, void *image,
+                                          int32_t *radii, const DgrRasterOptions *opt, void *stream);
+int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, const void *binning, uint64_t capacity_instances,
+                    int32_t staging, const void *image, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                    const DgrGaussianGrads *gout, const DgrRasterOptions *opt, void *stream);
+int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom, const void *binning, uint64_t capacity_instances,
+                          int32_t staging, const void *image, const int32_t *radii, const DgrImageGrads *gin,
+                          const DgrGaussianGrads *gout, const DgrRasterOptions *opt, void *stream);
+int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, const void *binning,
+                                uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii,
+                                const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views,
+                                const DgrRasterOptions *opt, void *stream);
+int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, const void *binning, uint64_t capacity_instances,
+                        int32_t staging, const void *image, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
+                        const DgrGaussianGrads *gout, void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances,
+                        const DgrRasterOptions *opt, void *stream);
+int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *geom, const void *binning, uint64_t capacity_instances,
+                              int32_t staging, const void *image, const int32_t *radii, const DgrImageGrads *gin,
+                              const DgrGaussianGrads *gout, void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances,
+                              const DgrRasterOptions *opt, void *stream);
+int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, const void *binning,
+                                    uint64_t capacity_instances, int32_t staging, const void *image, const int32_t *radii,
+                                    const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views, void *det_scratch,
+                                    uint64_t det_scratch_bytes, uint64_t instances, const DgrRasterOptions *opt, void *stream);
+
 /* Multi-GPU (view-sharded data parallelism, SURVEY.md §8e): all-reduce(sum) of the flat float32 gradient buffer over
  * NVLink with this library's own kernel.  The buffer lives in symmetric memory: peer_ptrs[w] (HOST array of `world` device
  * addresses) is rank w's copy mapped into this process; multicast_ptr, if non-zero, is the NVSwitch multicast address of

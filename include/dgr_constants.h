@@ -23,6 +23,7 @@
 #define DGR_ALPHA_MIN       (1.0f / 255.0f) /* UNVERIFIED-EXT contributions below this are skipped           */
 #define DGR_T_STOP          1e-4f       /* UNVERIFIED-EXT stop when T * (1 - alpha) < 1e-4                    */
 #define DGR_SH_OFFSET       0.5f        /* gs_renderer.py:793                                                 */
+#define DGR_AA_RATIO_FLOOR  2.5e-5f     /* UNVERIFIED-EXT anti-aliased mode: floor under det(cov2D) / det(cov2D + lowpass) */
 
 /* sh_utils.py:26-43 */
 #define DGR_SH_C0   0.28209479177387814f
