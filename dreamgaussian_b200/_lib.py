@@ -72,7 +72,20 @@ class DgrRasterOptions(ctypes.Structure):
     _fields_ = [("flags", ctypes.c_uint32)]
 
 
+class DgrCameraGrads(ctypes.Structure):
+    """Outputs of DGR_RASTER_CAMERA_GRADS (include/dgr_b200.h): [16] / [16] / [3], or [V,16] / [V,16] / [V,3] for the batched calls."""
+    _fields_ = [("dL_dviewmatrix", c_f32p), ("dL_dprojmatrix", c_f32p), ("dL_dcampos", c_f32p), ("scratch", ctypes.c_void_p),
+                ("scratch_bytes", ctypes.c_uint64)]
+
+
+class DgrRasterOptionsCamera(ctypes.Structure):
+    """DgrRasterOptions with its trailing `camera` member (read by the backward *_ex calls only with DGR_RASTER_CAMERA_GRADS);
+    pass it cast to POINTER(DgrRasterOptions).  DgrRasterOptions above is the flags-only prefix, which stays valid."""
+    _fields_ = [("flags", ctypes.c_uint32), ("camera", ctypes.POINTER(DgrCameraGrads))]
+
+
 RASTER_ANTIALIAS = 1                 # DGR_RASTER_ANTIALIAS
+RASTER_CAMERA_GRADS = 4              # DGR_RASTER_CAMERA_GRADS (backward *_ex calls only)
 
 VIEWS_MAX = 64                       # DGR_VIEWS_MAX
 VIEWS_MAX_RECORDS = 2 ** 31 - 1      # DGR_VIEWS_MAX_RECORDS: V x P
@@ -96,6 +109,7 @@ EXPORTS = (
     "dgr_forward_preprocess_ex", "dgr_views_forward_preprocess_ex", "dgr_views_mixed_forward_preprocess_ex",
     "dgr_backward_ex", "dgr_views_backward_ex", "dgr_views_mixed_backward_ex",
     "dgr_backward_det_ex", "dgr_views_backward_det_ex", "dgr_views_mixed_backward_det_ex",
+    "dgr_camera_grad_scratch_bytes",
 )
 
 _lib = None
@@ -220,6 +234,8 @@ def load():
         ex = getattr(lib, name + "_ex")
         ex.restype = ctypes.c_int
         ex.argtypes = list(getattr(lib, name).argtypes[:-1]) + [ctypes.POINTER(DgrRasterOptions), vp]
+    lib.dgr_camera_grad_scratch_bytes.restype = ctypes.c_size_t
+    lib.dgr_camera_grad_scratch_bytes.argtypes = [i32, i32]
     if lib.dgr_abi_version() != ABI_VERSION:
         raise RuntimeError("libdgr_b200.so ABI version mismatch")
     _lib = lib

@@ -18,6 +18,7 @@
 #include "../../include/dgr_b200.h"
 #include "dgr_backward.cuh"
 #include "dgr_binning.cuh"
+#include "dgr_camgrad.cuh"
 #include "dgr_collective.cuh"
 #include "dgr_densify.cuh"
 #include "dgr_det.cuh"
@@ -170,7 +171,28 @@ static_assert(DGR_RASTER_ANTIALIAS < 256u, "the known flags must fit the flags b
 
 int raster_flags(const DgrRasterOptions *opt, uint32_t *flags) {
     *flags = opt ? opt->flags : 0u;
+    if (*flags & DGR_RASTER_CAMERA_GRADS) return fail(-1, "DgrRasterOptions: DGR_RASTER_CAMERA_GRADS is backward-only (a forward call refuses it)");
     if (*flags & ~DGR_RASTER_ANTIALIAS) return fail(-1, "DgrRasterOptions: unknown flag bits");
+    return 0;
+}
+// The backward calls' options: the recorded / compared flags (DGR_RASTER_ANTIALIAS) and, with DGR_RASTER_CAMERA_GRADS, the camera
+// outputs (*cam; NULL without the bit).
+int raster_flags_bwd(const DgrRasterOptions *opt, uint32_t *flags, const DgrCameraGrads **cam) {
+    *flags = opt ? opt->flags : 0u;
+    *cam = nullptr;
+    if (*flags & ~(DGR_RASTER_ANTIALIAS | DGR_RASTER_CAMERA_GRADS)) return fail(-1, "DgrRasterOptions: unknown flag bits");
+    if (*flags & DGR_RASTER_CAMERA_GRADS) {
+        if (!opt->camera) return fail(-1, "DgrRasterOptions: DGR_RASTER_CAMERA_GRADS with camera == NULL");
+        *cam = opt->camera;
+    }
+    *flags &= DGR_RASTER_ANTIALIAS;
+    return 0;
+}
+int check_camera(const DgrCameraGrads *cam, int V, int P) {
+    if (!cam) return 0;
+    if (!cam->scratch) return fail(-1, "camera gradients: scratch is NULL");
+    if (cam->scratch_bytes < camera_grad_scratch_bytes(V, P))
+        return fail(-1, "camera gradients: scratch is smaller than dgr_camera_grad_scratch_bytes(V, P)");
     return 0;
 }
 int record_flags(char *image, const ImageLayout &IL, uint32_t flags, cudaStream_t st) {
@@ -241,6 +263,17 @@ void launch_pre_bwd(const DgrSettings *s, const DgrGaussians *g, const int *radi
     else launch(preprocess_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, 0, 0);
 }
 
+// camera gradients (dgr_camgrad.cuh): one CTA row per (256 Gaussians, view) into the caller's scratch
+template <int DEG, bool HAS_SH, bool HAS_COV, bool RAW>
+void launch_camera_bwd(int V, const ViewTable &vt, float2 tan0, const float *tanfov, float scale_modifier, const float *viewmatrix,
+                       const float *projmatrix, const float *campos, const DgrGaussians *g, const int *radii, const unsigned *touched,
+                       const float *grad_rec, float *rows, bool aa, cudaStream_t st) {
+    const dim3 grid((unsigned)((g->P + kPreThreads - 1) / kPreThreads), (unsigned)V);
+    launch_k(aa ? camera_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, true> : camera_bwd_kernel<DEG, HAS_SH, HAS_COV, RAW, false>, grid,
+             dim3(kPreThreads), 0, st, false, g->P, g->M, vt, tan0, tanfov, scale_modifier, viewmatrix, projmatrix, campos, g->means3D,
+             g->shs, g->shs_rest, g->scales, g->rotations, g->cov3D_precomp, radii, touched, grad_rec, rows);
+}
+
 #define DGR_DISPATCH(FN, ...)                                                                              \
     do {                                                                                                   \
         const bool sh_ = g->shs != nullptr, cov_ = g->cov3D_precomp != nullptr;                            \
@@ -258,6 +291,21 @@ void launch_pre_bwd(const DgrSettings *s, const DgrGaussians *g, const int *radi
             default: if (cov_) FN<3, true, true, false>(__VA_ARGS__); else FN<3, true, false, false>(__VA_ARGS__); break; \
         }                                                                                                  \
     } while (0)
+
+// The two camera-gradient kernels after the per-Gaussian backward of a checked call (S = DgrSettings or DgrViews).  tanfov = NULL:
+// single view, tan0 = (tanfovx, tanfovy).  An empty cloud launches only the reduction, which writes zeros.
+template <class S>
+int camera_grads(const S *s, const DgrGaussians *g, const DgrCameraGrads *cam, int V, const ViewTable &vt, float2 tan0, const float *tanfov,
+                 const int *radii, const unsigned *touched, const float *grad_rec, bool aa, cudaStream_t st) {
+    float *rows = reinterpret_cast<float *>(cam->scratch);
+    const int nblk = (g->P + kPreThreads - 1) / kPreThreads;
+    if (g->P > 0)
+        DGR_KERNEL("camera_bwd", st, s->debug, DGR_DISPATCH(launch_camera_bwd, V, vt, tan0, tanfov, s->scale_modifier, s->viewmatrix,
+                                                            s->projmatrix, s->campos, g, radii, touched, grad_rec, rows, aa, st));
+    DGR_KERNEL("camera_reduce", st, s->debug, launch_k(camera_reduce_kernel, dim3((unsigned)V), dim3(kCamReduceThreads), 0, st, false, nblk,
+                                                      (const float *)rows, cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos));
+    return 0;
+}
 
 __global__ void debug_geom_kernel(int P, const Rec *rec, const unsigned *touched, float *mean_px, float *depth, float *conic,
                                   float *rgb, int *aabb, unsigned *tiles_touched) {
@@ -658,18 +706,22 @@ static int flat_segs(int32_t n_seg, const int64_t *seg_off, const int32_t *seg_s
 // dgr_backward (det = NULL) and dgr_backward_det
 static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                            int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                           const DgrGaussianGrads *gout, const DetArgs *det, uint32_t flags, void *stream) {
+                           const DgrGaussianGrads *gout, const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, void *stream) {
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
+    if (int e = check_camera(cam, 1, g->P)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
     if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
         return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
     if (det)
         if (int e = check_det(*det, gout, capacity, g->P)) return e;
-    if (g->P == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    ViewTable vt1;                                   // the camera kernels' view table: one view of H x W
+    if (cam) { memset(&vt1, 0, sizeof(vt1)); vt1.H[0] = s->image_height; vt1.W[0] = s->image_width; }
+    if (g->P == 0)
+        return cam ? camera_grads(s, g, cam, 1, vt1, make_float2(s->tanfovx, s->tanfovy), nullptr, radii, nullptr, nullptr, false, st) : 0;
     if (!radii) return fail(-1, "radii is NULL");
     if (int e = check_push(gout->push, g->P)) return e;
-    cudaStream_t st = (cudaStream_t)stream;
     char *geom = (char *)geom_v;
     const char *binning = (const char *)binning_v, *image = (const char *)image_v;
     const int H = s->image_height, W = s->image_width;
@@ -733,6 +785,9 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
     }
     const bool aa = flags & DGR_RASTER_ANTIALIAS;
     DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, aa, st));
+    if (cam)
+        return camera_grads(s, g, cam, 1, vt1, make_float2(s->tanfovx, s->tanfovy), nullptr, radii,
+                            reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, aa, st);
     return 0;
 }
 
@@ -741,7 +796,7 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
                  const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_backward");
     (void)out_alpha;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, stream);
 }
 
 int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -750,11 +805,13 @@ int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, c
     NvtxRange nvtx_("dgr_backward_ex");
     (void)out_alpha;
     uint32_t flags = 0;
-    if (int e = raster_flags(opt, &flags)) return e;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, stream);
+    const DgrCameraGrads *cam = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, stream);
 }
 
 size_t dgr_det_scratch_bytes(uint64_t instances, int64_t records) { return DetLayout(instances, records).total; }
+size_t dgr_camera_grad_scratch_bytes(int32_t V, int32_t P) { return camera_grad_scratch_bytes(V, P); }
 
 int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                      int32_t staging, const void *image_v, const int32_t *radii, const float *out_alpha, const DgrImageGrads *gin,
@@ -762,7 +819,7 @@ int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom_v, 
     NvtxRange nvtx_("dgr_backward_det");
     (void)out_alpha;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, stream);
 }
 
 int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -772,9 +829,10 @@ int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_
     NvtxRange nvtx_("dgr_backward_det_ex");
     (void)out_alpha;
     uint32_t flags = 0;
-    if (int e = raster_flags(opt, &flags)) return e;
+    const DgrCameraGrads *cam = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, stream);
 }
 
 }  // extern "C"
@@ -998,12 +1056,13 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
 
 int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                    int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views,
-                   const DetArgs *det, uint32_t flags, void *stream) {
+                   const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, void *stream) {
     if (det)
         if (int e = check_det(*det, gout, capacity, (long long)g->P * s->V)) return e;
-    if (g->P == 0) return 0;
-    if (!radii) return fail(-1, "radii is NULL");
+    if (int e = check_camera(cam, s->V, g->P)) return e;
     cudaStream_t st = (cudaStream_t)stream;
+    if (g->P == 0) return cam ? camera_grads(s, g, cam, s->V, b.vt, make_float2(0.f, 0.f), s->tanfov, radii, nullptr, nullptr, false, st) : 0;
+    if (!radii) return fail(-1, "radii is NULL");
     char *geom = (char *)geom_v;
     const char *binning = (const char *)binning_v, *image = (const char *)image_v;
     const GeomLayout GL = GeomLayout::batch(g->P, b.tiles, s->V);
@@ -1048,6 +1107,9 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
     DGR_KERNEL("preprocess_views_bwd", st, s->debug,
                DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, b, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout,
                                   stats_views, aa, st));
+    if (cam)
+        return camera_grads(s, g, cam, s->V, b.vt, make_float2(0.f, 0.f), s->tanfov, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched),
+                            grad_rec, aa, st);
     return 0;
 }
 }  // namespace
@@ -1087,7 +1149,7 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
 
 static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                                const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
-                               const DetArgs *det, uint32_t flags, void *stream) {
+                               const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, void *stream) {
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1097,13 +1159,13 @@ static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *g
         return fail(-2, "views: the fused densification statistics are not supported by the batched call");
     if (int e = check_views_grads(gout)) return e;
     return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, det, flags,
-                          stream);
+                          cam, stream);
 }
 
 int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                        const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_views_backward");
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, stream);
 }
 
 int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1111,8 +1173,9 @@ int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v
                           const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_ex");
     uint32_t flags = 0;
-    if (int e = raster_flags(opt, &flags)) return e;
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, stream);
+    const DgrCameraGrads *cam = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, stream);
 }
 
 int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1120,7 +1183,7 @@ int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_
                            void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, stream);
 }
 
 int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1128,9 +1191,10 @@ int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *ge
                               void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_det_ex");
     uint32_t flags = 0;
-    if (int e = raster_flags(opt, &flags)) return e;
+    const DgrCameraGrads *cam = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, stream);
 }
 
 // ---- views of different sizes: image_hw = [V,2] (height, width) on the host ------------------------------------------------------
@@ -1178,7 +1242,8 @@ int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, c
 
 static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
                                 uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, uint32_t flags, void *stream) {
+                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, uint32_t flags,
+                                const DgrCameraGrads *cam, void *stream) {
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1192,7 +1257,7 @@ static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, cons
         return fail(-1, "views mixed: a densification statistic buffer is set but stats_views is 0");
     if (int e = check_views_grads(gout)) return e;
     return views_backward(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout,
-                          stats_views, det, flags, stream);
+                          stats_views, det, flags, cam, stream);
 }
 
 int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1200,7 +1265,7 @@ int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const D
                              const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward");
     return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, 0u,
-                                stream);
+                                nullptr, stream);
 }
 
 int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1208,9 +1273,10 @@ int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, cons
                                 const DgrGaussianGrads *gout, uint64_t stats_views, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_ex");
     uint32_t flags = 0;
-    if (int e = raster_flags(opt, &flags)) return e;
+    const DgrCameraGrads *cam = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
     return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, flags,
-                                stream);
+                                cam, stream);
 }
 
 int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1219,7 +1285,7 @@ int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, con
                                  uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, 0u, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, 0u, nullptr, stream);
 }
 
 int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1228,10 +1294,11 @@ int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, 
                                     uint64_t instances, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_det_ex");
     uint32_t flags = 0;
-    if (int e = raster_flags(opt, &flags)) return e;
+    const DgrCameraGrads *cam = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
     return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, flags,
-                                stream);
+                                cam, stream);
 }
 
 }  // extern "C"

@@ -172,10 +172,29 @@ forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modif
     return {color, st->radii, depth, alpha, st};
 }
 
-// grads: (means3D, means2D, shs | features_dc, colors, opacities, scales, rotations, cov3D, features_rest); undefined where not applicable
+// Camera gradients (DGR_RASTER_CAMERA_GRADS): appends dL/dviewmatrix, dL/dprojmatrix ([V,16] each, [16] for V = 0: single view)
+// and dL/dcampos ([V,3] / [3]) to g and returns the options of the backward call; without camera, the forward's options unchanged.
+struct CameraOut { DgrCameraGrads cg{}; DgrRasterOptions opt{0u, nullptr}; Tensor scratch; };
+void camera_out(bool camera, int64_t V, int64_t P, const DgrRasterOptions &fwd, const torch::TensorOptions &f32, std::vector<Tensor> &g,
+                CameraOut &c) {
+    c.opt = fwd;
+    if (!camera) return;
+    const std::vector<int64_t> s16 = V ? std::vector<int64_t>{V, 16} : std::vector<int64_t>{16};
+    const std::vector<int64_t> s3 = V ? std::vector<int64_t>{V, 3} : std::vector<int64_t>{3};
+    g.push_back(torch::empty(s16, f32)); g.push_back(torch::empty(s16, f32)); g.push_back(torch::empty(s3, f32));
+    c.scratch = torch::empty({(int64_t)dgr_camera_grad_scratch_bytes((int32_t)std::max<int64_t>(V, 1), (int32_t)P)}, f32.dtype(torch::kUInt8));
+    const size_t n = g.size();
+    c.cg = DgrCameraGrads{g[n - 3].data_ptr<float>(), g[n - 2].data_ptr<float>(), g[n - 1].data_ptr<float>(), c.scratch.data_ptr(),
+                          (uint64_t)c.scratch.numel()};
+    c.opt.flags |= DGR_RASTER_CAMERA_GRADS;
+    c.opt.camera = &c.cg;
+}
+
+// grads: (means3D, means2D, shs | features_dc, colors, opacities, scales, rotations, cov3D, features_rest); undefined where not applicable;
+// camera: + (dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3])
 std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA, bool accumulate,
                              const std::vector<OptTensor> &out, const OptTensor &xyz_gradient_accum, const OptTensor &denom,
-                             const OptTensor &max_radii2D, int64_t push_addr) {
+                             const OptTensor &max_radii2D, int64_t push_addr, bool camera) {
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     const int64_t P = st->g.P, M = st->g.M;
     const auto f32 = st->means3D.options();
@@ -199,16 +218,18 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
     DgrGaussianGrads gout{gp(0), gp(1), gp(2), gp(3), gp(4), gp(5), gp(6), gp(7), accumulate ? 1 : 0, gp(8),
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D),
                           reinterpret_cast<const DgrPeerPush *>(push_addr)};      // host struct kept alive by the caller (0 = none)
+    CameraOut cam;
+    camera_out(camera, 0, P, st->opt, f32, g, cam);
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
     if (at::globalContext().deterministicAlgorithms()) {
         Tensor det = det_scratch(st->n_inst, P, f32);
         check(dgr_backward_det_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
                                   st->image.data_ptr(), st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, det.data_ptr(),
-                                  (uint64_t)det.numel(), (uint64_t)st->n_inst, &st->opt, stream));
+                                  (uint64_t)det.numel(), (uint64_t)st->n_inst, &cam.opt, stream));
         return g;
     }
     check(dgr_backward_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging, st->image.data_ptr(),
-                          st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, &st->opt, stream));
+                          st->radii.data_ptr<int32_t>(), nullptr, &gin, &gout, &cam.opt, stream));
     return g;
 }
 
@@ -390,10 +411,11 @@ views_mixed_forward(const std::vector<int32_t> &image_hw, double scale_modifier,
 }
 
 // grads: (means3D, means2D [V,P,3], shs | features_dc, opacities, scales, rotations, features_rest); the per-Gaussian ones summed over views.
-// Mixed sizes only: the densification statistics of the views in stats_views.
+// Mixed sizes only: the densification statistics of the views in stats_views.  camera: + each view's (dL/dviewmatrix [V,16],
+// dL/dprojmatrix [V,16], dL/dcampos [V,3]).
 std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
                                         bool accumulate, const std::vector<OptTensor> &out, const OptTensor &xyz_gradient_accum,
-                                        const OptTensor &denom, const OptTensor &max_radii2D, uint64_t stats_views) {
+                                        const OptTensor &denom, const OptTensor &max_radii2D, uint64_t stats_views, bool camera) {
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     const int64_t P = st->g.P, M = st->g.M, V = st->s.V;
     const auto f32 = st->means3D.options();
@@ -412,6 +434,8 @@ std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, c
     DgrImageGrads gin{fptr(c), fptr(d), fptr(a)};
     DgrGaussianGrads gout{gp(0), gp(1), gp(2), nullptr, gp(3), gp(4), gp(5), nullptr, accumulate ? 1 : 0, gp(6),
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D), nullptr};
+    CameraOut cam;
+    camera_out(camera, V, P, st->opt, f32, g, cam);
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
     if (at::globalContext().deterministicAlgorithms()) {
         Tensor det = det_scratch(st->n_inst, P * V, f32);
@@ -419,26 +443,26 @@ std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, c
         if (!st->hw.empty())
             check(dgr_views_mixed_backward_det_ex(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(),
                                                   (uint64_t)st->capacity, st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin,
-                                                  &gout, stats_views, det.data_ptr(), bytes, n, &st->opt, stream));
+                                                  &gout, stats_views, det.data_ptr(), bytes, n, &cam.opt, stream));
         else
             check(dgr_views_backward_det_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
-                                            st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, det.data_ptr(), bytes, n, &st->opt,
+                                            st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, det.data_ptr(), bytes, n, &cam.opt,
                                             stream));
         return g;
     }
     if (!st->hw.empty())
         check(dgr_views_mixed_backward_ex(&st->s, st->hw.data(), &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity,
-                                          st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views, &st->opt,
+                                          st->staging, st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, stats_views, &cam.opt,
                                           stream));
     else
         check(dgr_views_backward_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)st->capacity, st->staging,
-                                    st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, &st->opt, stream));
+                                    st->image.data_ptr(), st->radii.data_ptr<int32_t>(), &gin, &gout, &cam.opt, stream));
     return g;
 }
 
 std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
-                                   bool accumulate, const std::vector<OptTensor> &out) {
-    return views_backward_impl(st, gC, gD, gA, accumulate, out, c10::nullopt, c10::nullopt, c10::nullopt, 0);
+                                   bool accumulate, const std::vector<OptTensor> &out, bool camera) {
+    return views_backward_impl(st, gC, gD, gA, accumulate, out, c10::nullopt, c10::nullopt, c10::nullopt, 0, camera);
 }
 
 }  // namespace
@@ -454,7 +478,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("scales"), py::arg("rots"), py::arg("cov3D"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("backward", &backward, "backward through the C ABI", pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"),
           pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"),
-          pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0);
+          pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0, pybind11::arg("camera") = false);
     pybind11::class_<ViewsState, std::shared_ptr<ViewsState>>(m, "ViewsState")
         .def_readonly("capacity", &ViewsState::capacity)
         .def_readonly("num_rendered", &ViewsState::n_inst);
@@ -462,14 +486,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("debug"), py::arg("tanfov"), py::arg("bg"), py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"),
           py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("views_backward", &views_backward, "backward of the batched-camera call through the C ABI", pybind11::arg("state"),
-          pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"));
+          pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"),
+          pybind11::arg("camera") = false);
     m.def("views_mixed_forward", &views_mixed_forward, "both forward stages of the batched call with a size per view through the C ABI",
           py::arg("image_hw"), py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("debug"), py::arg("tanfov"), py::arg("bg"), py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"),
           py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("views_mixed_backward", &views_backward_impl, "backward of the batched call with a size per view through the C ABI",
           pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"),
           pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"), pybind11::arg("denom"), pybind11::arg("max_radii2D"),
-          pybind11::arg("stats_views"));
+          pybind11::arg("stats_views"), pybind11::arg("camera") = false);
     m.def("set_views_mixed_hint", [](int dev, int64_t P, const std::vector<int32_t> &hw, int64_t cap, bool big) {
         std::lock_guard<std::mutex> lk(g_mu); g_views_mixed_hints[views_mixed_hint_key(dev, P, hw)] = Hint{cap, big}; });
     m.def("get_views_mixed_hint", [](int dev, int64_t P, const std::vector<int32_t> &hw) -> pybind11::object {

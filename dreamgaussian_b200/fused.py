@@ -36,7 +36,8 @@ class DensifyStats:
 class _RasterizeRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, means2D, features_dc, features_rest, opacity_raw, scaling_raw, rotation_raw, raster_settings, stats,
-                antialiasing=False):
+                antialiasing=False, *cams):
+        ctx.cams = cams                  # (viewmatrix, projmatrix, campos) when their gradient is asked for
         if _r._FAST is not None:
             color, radii, depth, alpha, state = _r.forward_impl(raster_settings, xyz, features_dc, None, opacity_raw, scaling_raw, rotation_raw,
                                                                 None, sh_rest=features_rest, activations=True, antialiasing=antialiasing)
@@ -63,10 +64,13 @@ class _RasterizeRaw(torch.autograd.Function):
         if getattr(state, "stats_applied", False):
             ctx.stats = None
         state.stats_applied = True
+        needs = ctx.needs_input_grad[10:]
+        cam_needed = any(needs)
         if state.fast is not None:
             stats = ctx.stats.as_tuple() if ctx.stats is not None else (None, None, None)
-            g = _r._FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *stats)
-            return g[0], g[1], g[2], g[8], g[4], g[5], g[6], None, None, None
+            g = _r._FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *stats, camera=cam_needed)
+            cg = _r._camera_input_grads(ctx.cams, needs, g[9:12]) if cam_needed else [None] * len(ctx.cams)
+            return (g[0], g[1], g[2], g[8], g[4], g[5], g[6], None, None, None, *cg)
         xyz, dc, _, op, sc, rot, _, rest = state.tensors
         P = state.frame.P
         f32 = dict(dtype=torch.float32, device=xyz.device)
@@ -78,14 +82,17 @@ class _RasterizeRaw(torch.autograd.Function):
         d_rest = torch.empty(rest.shape, **f32) if rest is not None else None
         d_op, d_sc, d_rot = torch.empty((P, 1), **f32), torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
         stats = ctx.stats.as_tuple() if ctx.stats is not None else None
-        _r.backward_impl(state, gC, gD, gA, d_xyz, d_m2d, d_dc, None, d_op, d_sc, d_rot, None, d_sh_rest=d_rest, densify=stats)
-        return d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, None
+        camera = _r._camera_outputs(0, xyz.device) if cam_needed else None
+        _r.backward_impl(state, gC, gD, gA, d_xyz, d_m2d, d_dc, None, d_op, d_sc, d_rot, None, d_sh_rest=d_rest, densify=stats, camera=camera)
+        cg = _r._camera_input_grads(ctx.cams, needs, camera) if cam_needed else [None] * len(ctx.cams)
+        return (d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, None, *cg)
 
 
 class FusedGaussianRasterizer(nn.Module):
     """`GaussianRasterizer` for raw parameters.  forward(xyz, features_dc, features_rest, opacity, scaling, rotation,
     means2D=None, stats=None) -> (color [3,H,W], radii int32 [P], depth [1,H,W], alpha [1,H,W]); `stats` (DensifyStats) is
-    updated during the backward.  antialiasing: as GaussianRasterizer (the 2D Mip filter with opacity compensation)."""
+    updated during the backward.  antialiasing: as GaussianRasterizer (the 2D Mip filter with opacity compensation).  Camera
+    tensors of the settings that require grad receive their gradient, as with GaussianRasterizer."""
 
     def __init__(self, raster_settings: _r.GaussianRasterizationSettings, antialiasing: bool = False):
         super().__init__()
@@ -97,7 +104,7 @@ class FusedGaussianRasterizer(nn.Module):
         if means2D is None:
             means2D = torch.zeros_like(xyz, requires_grad=xyz.requires_grad)
         return _RasterizeRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, self.raster_settings, stats,
-                                   self.antialiasing)
+                                   self.antialiasing, *_r._camera_tensors([self.raster_settings]))
 
 
 def render_gaussian_model(gaussians, raster_settings, stats: Optional[DensifyStats] = None, antialiasing: bool = False):
@@ -114,7 +121,9 @@ def render_gaussian_model(gaussians, raster_settings, stats: Optional[DensifySta
 
 class _RasterizeViewsRaw(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, xyz, means2D, features_dc, features_rest, opacity_raw, scaling_raw, rotation_raw, settings_list, antialiasing=False):
+    def forward(ctx, xyz, means2D, features_dc, features_rest, opacity_raw, scaling_raw, rotation_raw, settings_list, antialiasing=False,
+                *cams):
+        ctx.cams = cams
         xyz = _r._dev_f32(xyz, "xyz")
         dc = _r._dev_f32(features_dc, "features_dc")
         rest = _r._opt(features_rest, "features_rest")
@@ -129,8 +138,9 @@ class _RasterizeViewsRaw(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
-        d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot = _r._views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=True)
-        return d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None
+        (d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot), cg = _r._views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha,
+                                                                                                True, 9)
+        return (d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, *cg)
 
 
 def rasterize_views_raw(settings_list, xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, antialiasing=False):
@@ -141,13 +151,15 @@ def rasterize_views_raw(settings_list, xyz, means2D, features_dc, features_rest,
     settings_list = _r._check_views_settings(settings_list)
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), xyz.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
-    return _RasterizeViewsRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, settings_list, bool(antialiasing))
+    return _RasterizeViewsRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, settings_list, bool(antialiasing),
+                                    *_r._camera_tensors(settings_list))
 
 
 class _RasterizeViewsMixedRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, means2D, features_dc, features_rest, opacity_raw, scaling_raw, rotation_raw, settings_list, stats, stats_mask,
-                antialiasing=False):
+                antialiasing=False, *cams):
+        ctx.cams = cams
         xyz = _r._dev_f32(xyz, "xyz")
         dc = _r._dev_f32(features_dc, "features_dc")
         rest = _r._opt(features_rest, "features_rest")
@@ -167,9 +179,9 @@ class _RasterizeViewsMixedRaw(torch.autograd.Function):
         if getattr(state, "stats_applied", False):
             ctx.stats = None
         state.stats_applied = True
-        d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot = _r._views_grads(state, grad_color, grad_depth, grad_alpha, raw=True, stats=ctx.stats,
-                                                                        stats_views=ctx.stats_mask)
-        return d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, None, None
+        (d_xyz, d_m2d, d_dc, d_rest, d_op, d_sc, d_rot), cg = _r._views_backward_with_cameras(
+            ctx, grad_color, grad_depth, grad_alpha, True, 11, stats=ctx.stats, stats_views=ctx.stats_mask)
+        return (d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, None, None, *cg)
 
 
 def rasterize_views_mixed_raw(settings_list, xyz, means2D, features_dc, features_rest, opacity, scaling, rotation, stats=None,
@@ -184,6 +196,7 @@ def rasterize_views_mixed_raw(settings_list, xyz, means2D, features_dc, features
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
     mask = _r._stats_mask(stats_views, len(settings_list))
     color, radii, depth, alpha = _RasterizeViewsMixedRaw.apply(xyz, means2D, features_dc, features_rest, opacity, scaling, rotation,
-                                                               settings_list, stats if mask else None, mask, bool(antialiasing))
+                                                               settings_list, stats if mask else None, mask, bool(antialiasing),
+                                                               *_r._camera_tensors(settings_list))
     colors, depths, alphas = _r.split_views(settings_list, color, depth, alpha)
     return colors, radii, depths, alphas

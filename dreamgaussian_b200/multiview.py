@@ -63,6 +63,7 @@ class ViewShardedRasterizer:
     """Forward + backward of this rank's views with gradient accumulation, then one all-reduce.
 
     params: dict(means3D, shs, opacities, scales, rotations) of CUDA float32 tensors (replicated on every rank).
+    The cameras are constants here: unlike the autograd render calls, this path computes no camera gradients.
     """
 
     def __init__(self, P: int, M: int, device, process_group=None, peer_allreduce: bool = True):

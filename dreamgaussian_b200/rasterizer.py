@@ -170,6 +170,55 @@ def _raster_opts(antialiasing):
     return ctypes.byref(_lib.DgrRasterOptions(_lib.RASTER_ANTIALIAS if antialiasing else 0))
 
 
+def _backward_opts(antialiasing, camera, V, P, dev):
+    """The DgrRasterOptions argument of a backward *_ex call.  camera = (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos) float32 outputs
+    ([16], [16], [3] or [V,16], [V,16], [V,3]) or None; with them, DGR_RASTER_CAMERA_GRADS and its scratch (the returned pointer
+    keeps the option structs alive, the scratch stays alive until the call returns)."""
+    if camera is None:
+        return _raster_opts(antialiasing), None
+    lib = _lib.load()
+    scratch = torch.empty((lib.dgr_camera_grad_scratch_bytes(int(V), int(P)),), dtype=torch.uint8, device=dev)
+    cg = _lib.DgrCameraGrads(*(_ptr(t) for t in camera), _ptr(scratch), scratch.numel())
+    opt = _lib.DgrRasterOptionsCamera((_lib.RASTER_ANTIALIAS if antialiasing else 0) | _lib.RASTER_CAMERA_GRADS, ctypes.pointer(cg))
+    return ctypes.cast(ctypes.pointer(opt), ctypes.POINTER(_lib.DgrRasterOptions)), scratch
+
+
+# ---- camera gradients (DGR_RASTER_CAMERA_GRADS) -----------------------------------------------------------------------------
+# The settings are a non-tensor argument of the autograd functions; when grad mode is on and a camera tensor of the settings
+# requires grad, the calls below hand every view's (viewmatrix, projmatrix, campos) to the function as extra tensor inputs, and
+# its backward returns their gradients (the C ABI's per-view [16] / [16] / [3]) in each tensor's own shape and dtype.
+def _camera_tensors(settings_list):
+    """() unless grad mode is on and some viewmatrix / projmatrix / campos of the settings requires grad; else every view's
+    (viewmatrix, projmatrix, campos), flattened in view order."""
+    if not torch.is_grad_enabled():
+        return ()
+    flat = tuple(t for s in settings_list for t in (s.viewmatrix, s.projmatrix, s.campos))
+    if not any(isinstance(t, torch.Tensor) and t.requires_grad for t in flat):
+        return ()
+    return flat
+
+
+def _camera_outputs(V, dev):
+    """Output tensors of the camera gradients: [V,16], [V,16], [V,3] (V = 0: single view, [16], [16], [3])."""
+    f32 = dict(dtype=torch.float32, device=dev)
+    lead = (V,) if V else ()
+    return torch.empty(lead + (16,), **f32), torch.empty(lead + (16,), **f32), torch.empty(lead + (3,), **f32)
+
+
+def _camera_input_grads(cams, needs, grads):
+    """grads = (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos), per view or single -> the gradients of the flattened camera inputs
+    `cams` (None where needs is False), each in its input's shape and dtype."""
+    out = []
+    for i, t in enumerate(cams):
+        if not needs[i] or not isinstance(t, torch.Tensor):
+            out.append(None)
+            continue
+        g = grads[i % 3]
+        g = g.reshape(-1, g.shape[-1])[i // 3]
+        out.append(g.reshape(t.shape).to(dtype=t.dtype, device=t.device))
+    return out
+
+
 class ForwardState:
     """Everything one forward leaves behind for its backward (upstream: ctx + geom/binning/img buffers)."""
     __slots__ = ("rs", "frame", "num_rendered", "capacity", "staging", "geom", "binning", "image", "radii", "alpha", "tensors",
@@ -259,15 +308,19 @@ def _host_sync_objects(dev):
 
 
 def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot,
-                  d_cov, accumulate=False, d_sh_rest=None, densify=None, push=None):
+                  d_cov, accumulate=False, d_sh_rest=None, densify=None, push=None, camera=None):
     """Runs the backward through the C ABI, writing (or accumulating) into the given gradient tensors.
     densify = (xyz_gradient_accum, denom, max_radii2D) float32 [P] tensors (any may be None) updated in the same kernel.
-    push = a _lib.DgrPeerPush (multi-GPU: rows of Gaussians another rank owns go straight to that rank, include/dgr_b200.h)."""
+    push = a _lib.DgrPeerPush (multi-GPU: rows of Gaussians another rank owns go straight to that rank, include/dgr_b200.h).
+    camera = (dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3]) float32 tensors, written (never accumulated), or None."""
     push_addr = ctypes.addressof(push) if push is not None else 0
     if state.fast is not None:
-        _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate),
-                       [d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, d_sh_rest], *(densify or (None, None, None)),
-                       push_addr)
+        g = _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate),
+                           [d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, d_sh_rest], *(densify or (None, None, None)),
+                           push_addr, camera=camera is not None)
+        if camera is not None:
+            for dst, src in zip(camera, g[9:12]):
+                dst.copy_(src)
         return
     lib = _lib.load()
     fr = state.frame
@@ -280,12 +333,12 @@ def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2
         args = (ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(state.geom), _ptr(state.binning),
                 ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii), _ptr(state.alpha),
                 ctypes.byref(gin), ctypes.byref(gout))
+        opts, _scratch = _backward_opts(state.antialiasing, camera, 1, fr.P, dev)
         if torch.are_deterministic_algorithms_enabled():
             det = _det_scratch(lib, state.num_rendered, fr.P, dev)
-            _lib.check(lib.dgr_backward_det_ex(*args, *_det_args(det, state.num_rendered), _raster_opts(state.antialiasing),
-                                               _stream_ptr(dev)))
+            _lib.check(lib.dgr_backward_det_ex(*args, *_det_args(det, state.num_rendered), opts, _stream_ptr(dev)))
         else:
-            _lib.check(lib.dgr_backward_ex(*args, _raster_opts(state.antialiasing), _stream_ptr(dev)))
+            _lib.check(lib.dgr_backward_ex(*args, opts, _stream_ptr(dev)))
 
 
 def _det_scratch(lib, instances, records, dev):
@@ -301,7 +354,8 @@ def _det_args(det, instances):
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
-                antialiasing=False):
+                antialiasing=False, *cams):
+        ctx.cams = cams                  # (viewmatrix, projmatrix, campos) when their gradient is asked for (_camera_tensors)
         means3D = _dev_f32(means3D, "means3D")
         opacities = _dev_f32(opacities, "opacities")
         sh, colors_precomp = _opt(sh, "shs"), _opt(colors_precomp, "colors_precomp")
@@ -315,9 +369,13 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
         state = ctx.state
+        cams = ctx.cams
+        cam_needed = any(ctx.needs_input_grad[10:])
         if state.fast is not None:
-            g = _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], None, None, None)      # undefined -> None
-            return g[0], g[1], g[2], g[3], g[4], g[5], g[6], g[7], None, None
+            g = _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], None, None, None,
+                               camera=cam_needed)      # undefined -> None
+            cg = _camera_input_grads(cams, ctx.needs_input_grad[10:], g[9:12]) if cam_needed else [None] * len(cams)
+            return (g[0], g[1], g[2], g[3], g[4], g[5], g[6], g[7], None, None, *cg)
         means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, _ = state.tensors
         dev = means3D.device
         P, M = state.frame.P, state.frame.M
@@ -333,16 +391,19 @@ class _RasterizeGaussians(torch.autograd.Function):
         d_scales = torch.empty((P, 3), **f32) if scales is not None else None
         d_rot = torch.empty((P, 4), **f32) if rotations is not None else None
         d_cov = torch.empty((P, 6), **f32) if cov3D is not None else None
-        backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov)
+        camera = _camera_outputs(0, dev) if cam_needed else None
+        backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, camera=camera)
+        cg = _camera_input_grads(cams, ctx.needs_input_grad[10:], camera) if cam_needed else [None] * len(cams)
         # ctx.state stays: a retain_graph backward runs again from the same buffers (they go away with the graph node)
-        return d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, None, None
+        return (d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, None, None, *cg)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
                         antialiasing=False):
-    """antialiasing=True: the 2D Mip filter with opacity compensation (Mip-Splatting), DGR_RASTER_ANTIALIAS of include/dgr_b200.h."""
+    """antialiasing=True: the 2D Mip filter with opacity compensation (Mip-Splatting), DGR_RASTER_ANTIALIAS of include/dgr_b200.h.
+    A viewmatrix / projmatrix / campos of raster_settings that requires grad receives its gradient (DGR_RASTER_CAMERA_GRADS)."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                     raster_settings, bool(antialiasing))
+                                     raster_settings, bool(antialiasing), *_camera_tensors([raster_settings]))
 
 
 class GaussianRasterizer(nn.Module):
@@ -570,17 +631,21 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
 
 
 def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot,
-                        accumulate=False, d_sh_rest=None, densify=None, stats_views=0):
+                        accumulate=False, d_sh_rest=None, densify=None, stats_views=0, camera=None):
     """Backward of a batched forward: the per-Gaussian gradients are the sums over the views (written, or added with
     accumulate); d_means2D is per view, [V,P,3].  Mixed-size forwards only: densify = (xyz_gradient_accum, denom, max_radii2D)
-    float32 [P] tensors (any may be None), updated for the views whose bit is set in the stats_views mask."""
+    float32 [P] tensors (any may be None), updated for the views whose bit is set in the stats_views mask.
+    camera = (dL/dviewmatrix [V,16], dL/dprojmatrix [V,16], dL/dcampos [V,3]) float32 tensors, each view's own, or None."""
     if state.fast is not None:
         outs = [d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest]
         if state.mixed:
-            _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs, *(densify or (None, None, None)),
-                                       int(stats_views))
+            g = _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs,
+                                           *(densify or (None, None, None)), int(stats_views), camera=camera is not None)
         else:
-            _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs)
+            g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs, camera=camera is not None)
+        if camera is not None:
+            for dst, src in zip(camera, g[7:10]):
+                dst.copy_(src)
         return
     lib = _lib.load()
     vw = state.views
@@ -592,7 +657,7 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
                                      *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), None)
         common = (ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning), ctypes.c_uint64(state.capacity), state.staging,
                   _ptr(state.image), _ptr(state.radii), ctypes.byref(gin), ctypes.byref(gout))
-        opts = _raster_opts(state.antialiasing)
+        opts, _scratch = _backward_opts(state.antialiasing, camera, vw.V, vw.P, dev)
         if torch.are_deterministic_algorithms_enabled():
             det = _det_scratch(lib, state.num_rendered, vw.P * vw.V, dev)
             if state.mixed:
@@ -609,17 +674,19 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
             _lib.check(lib.dgr_views_backward_ex(ctypes.byref(vw.settings), *common, opts, _stream_ptr(dev)))
 
 
-def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, stats_views=0):
-    """-> (means3D, means2D [V,P,3], shs | features_dc, features_rest, opacities, scales, rotations) gradients.
+def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, stats_views=0, camera=False):
+    """-> (means3D, means2D [V,P,3], shs | features_dc, features_rest, opacities, scales, rotations) gradients, and with camera=True
+    also (dL/dviewmatrix [V,16], dL/dprojmatrix [V,16], dL/dcampos [V,3]) as an 8th element.
     stats (DensifyStats) / stats_views (bit mask): the densification statistics of a mixed-size forward."""
     densify = stats.as_tuple() if stats is not None else None
     if state.fast is not None:
         if state.mixed:
             g = _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *(densify or (None, None, None)),
-                                           int(stats_views) if densify is not None else 0)
+                                           int(stats_views) if densify is not None else 0, camera=bool(camera))
         else:
-            g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [])       # undefined -> None
-        return g[0], g[1], g[2], g[6], g[3], g[4], g[5]
+            g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], camera=bool(camera))   # undefined -> None
+        out = (g[0], g[1], g[2], g[6], g[3], g[4], g[5])
+        return out + (tuple(g[7:10]),) if camera else out
     means3D, sh, opacities, scales, rotations, sh_rest = state.tensors
     vw = state.views
     P, M, V = vw.P, vw.M, vw.V
@@ -631,14 +698,27 @@ def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, sta
     d_sh = torch.empty((P, 1 if raw else M, 3), **f32)
     d_rest = torch.empty(sh_rest.shape, **f32) if (raw and sh_rest is not None) else None
     d_scales, d_rot = torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
+    cam = _camera_outputs(V, means3D.device) if camera else None
     views_backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest=d_rest, densify=densify,
-                        stats_views=stats_views if densify is not None else 0)
-    return d_means3D, d_means2D, d_sh, d_rest, d_opac, d_scales, d_rot
+                        stats_views=stats_views if densify is not None else 0, camera=cam)
+    out = (d_means3D, d_means2D, d_sh, d_rest, d_opac, d_scales, d_rot)
+    return out + (cam,) if camera else out
+
+
+def _views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha, raw, first_cam, **kw):
+    """_views_grads for a batched autograd function whose camera inputs (if any) start at input index first_cam -> (the 7
+    per-Gaussian gradients, the list of camera-input gradients)."""
+    needs = ctx.needs_input_grad[first_cam:]
+    cam_needed = any(needs)
+    r = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=raw, camera=cam_needed, **kw)
+    cg = _camera_input_grads(ctx.cams, needs, r[7]) if cam_needed else [None] * len(ctx.cams)
+    return r[:7], cg
 
 
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False, *cams):
+        ctx.cams = cams
         means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
         sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
         color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
@@ -649,9 +729,10 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
-        d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=False)
+        (d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot), cg = _views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha,
+                                                                                                      False, 8)
         # ctx.state stays: a retain_graph backward runs again from the same buffers.  means2D may be None (no per-view gradient wanted)
-        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None
+        return (d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None, *cg)
 
 
 def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False):
@@ -660,11 +741,13 @@ def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rot
     Returns (color [V,3,H,W], radii int32 [V,P], depth [V,1,H,W], alpha [V,1,H,W]); view v equals what GaussianRasterizer
     returns for camera v.  The gradients of means3D / shs / opacities / scales / rotations are summed over the views;
     means2D is [V,P,3] (e.g. zeros with requires_grad) or None: its gradient is per view, for densification.  SH colours and
-    scale / rotation inputs only; no CPU path.  antialiasing: as GaussianRasterizer."""
+    scale / rotation inputs only; no CPU path.  antialiasing: as GaussianRasterizer.  A camera tensor of a settings entry that
+    requires grad receives that view's own gradient (DGR_RASTER_CAMERA_GRADS)."""
     settings_list = _check_views_settings(settings_list)
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
-    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list, bool(antialiasing))
+    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list, bool(antialiasing),
+                                 *_camera_tensors(settings_list))
 
 
 class GaussianViewsRasterizer(nn.Module):
@@ -698,7 +781,8 @@ def split_views(settings_list, color, depth, alpha):
 
 class _RasterizeViewsMixed(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False, *cams):
+        ctx.cams = cams
         means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
         sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
         color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, mixed=True,
@@ -709,8 +793,9 @@ class _RasterizeViewsMixed(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
-        d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot = _views_grads(ctx.state, grad_color, grad_depth, grad_alpha, raw=False)
-        return d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None
+        (d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot), cg = _views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha,
+                                                                                                      False, 8)
+        return (d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None, *cg)
 
 
 def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False):
@@ -723,6 +808,6 @@ def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scale
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
     color, radii, depth, alpha = _RasterizeViewsMixed.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list,
-                                                            bool(antialiasing))
+                                                            bool(antialiasing), *_camera_tensors(settings_list))
     colors, depths, alphas = split_views(settings_list, color, depth, alpha)
     return colors, radii, depths, alphas

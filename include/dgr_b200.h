@@ -307,8 +307,35 @@ int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, con
  * Cost: only the per-Gaussian forward and backward kernels differ (their *_aa_kernel variants: a few dozen FLOPs and a square
  * root per Gaussian and view); the binning, sort and render kernels are those of the default mode (DESIGN.md §4 has the times). */
 #define DGR_RASTER_ANTIALIAS 1u
+/* == Camera gradients (DGR_RASTER_CAMERA_GRADS, backward *_ex calls only) ==
+ * The backward also returns dL/dviewmatrix [16] (the layout of DgrSettings.viewmatrix: row-major, p_view = [p,1] V),
+ * dL/dprojmatrix [16] and dL/dcampos [3] of the render; for dgr_views_* and dgr_views_mixed_* [V,16], [V,16] and [V,3], each view's
+ * own.  They are the exact chain rule of the forward as the per-Gaussian backward differentiates it: the cull decisions, radius,
+ * tile rectangle, opacity-aware box, the 0.3 low-pass, the eigenvalue floor and the clamped tx'/ty' inside J are constants, and
+ * min(0.99, .) is straight-through.  Column 3 of dL/dviewmatrix and column 2 of dL/dprojmatrix are 0 (the forward never reads
+ * them); dL/dcampos is 0 with colors_precomp and at sh_degree 0.  With DGR_RASTER_ANTIALIAS the opacity-compensation gradient
+ * is included.  tanfovx / tanfovy and bg get no gradient.
+ * Any of the three output pointers may be NULL; the others are always written, never accumulated, whatever
+ * DgrGaussianGrads.accumulate says.  scratch: device memory of at least dgr_camera_grad_scratch_bytes(V, P) bytes (V = 1 for
+ * the single-view calls).  No float atomics: each CTA of the extra kernel (camera_bwd) reduces its partials in a fixed order and
+ * camera_reduce adds the CTAs' rows in order, so the gradients are bit-reproducible whenever the moments are (the *_det calls).
+ * Refused before any device work: the bit with camera == NULL, scratch that is NULL or too small, and the bit on a forward *_ex
+ * call.  The flags a forward records, and the debug comparison of a backward's flags with them, cover DGR_RASTER_ANTIALIAS only.
+ * Without the bit a call launches exactly the kernels it launched before the bit existed; `camera` is read only with it, so a
+ * caller's DgrRasterOptions that ends after `flags` stays valid.  Bit 2u stays unknown (refused), so a flags-only struct can
+ * never be read past its end.  Cost: two kernels after the per-Gaussian backward (DESIGN.md §4). */
+#define DGR_RASTER_CAMERA_GRADS 4u
+typedef struct DgrCameraGrads {
+    float *dL_dviewmatrix;   /* [16] or [V,16], or NULL */
+    float *dL_dprojmatrix;   /* [16] or [V,16], or NULL */
+    float *dL_dcampos;       /* [3] or [V,3], or NULL */
+    void *scratch;           /* device, >= dgr_camera_grad_scratch_bytes(V, P) */
+    uint64_t scratch_bytes;
+} DgrCameraGrads;
+size_t dgr_camera_grad_scratch_bytes(int32_t V, int32_t P);
 typedef struct DgrRasterOptions {
     uint32_t flags;          /* DGR_RASTER_* bits */
+    const DgrCameraGrads *camera;   /* read only when flags has DGR_RASTER_CAMERA_GRADS */
 } DgrRasterOptions;
 int dgr_forward_preprocess_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii,
                               const DgrRasterOptions *opt, void *stream);
