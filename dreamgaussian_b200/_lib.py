@@ -84,8 +84,15 @@ class DgrRasterOptionsCamera(ctypes.Structure):
     _fields_ = [("flags", ctypes.c_uint32), ("camera", ctypes.POINTER(DgrCameraGrads))]
 
 
+class DgrRasterOptionsFull(ctypes.Structure):
+    """DgrRasterOptions with both trailing members: `camera` (read only with DGR_RASTER_CAMERA_GRADS) and `xyz_gradient_accum_abs`
+    (read only with DGR_RASTER_ABS_GRAD); pass it cast to POINTER(DgrRasterOptions)."""
+    _fields_ = [("flags", ctypes.c_uint32), ("camera", ctypes.POINTER(DgrCameraGrads)), ("xyz_gradient_accum_abs", c_f32p)]
+
+
 RASTER_ANTIALIAS = 1                 # DGR_RASTER_ANTIALIAS
 RASTER_CAMERA_GRADS = 4              # DGR_RASTER_CAMERA_GRADS (backward *_ex calls only)
+RASTER_ABS_GRAD = 16                 # DGR_RASTER_ABS_GRAD (backward *_ex calls only)
 
 VIEWS_MAX = 64                       # DGR_VIEWS_MAX
 VIEWS_MAX_RECORDS = 2 ** 31 - 1      # DGR_VIEWS_MAX_RECORDS: V x P
@@ -109,7 +116,7 @@ EXPORTS = (
     "dgr_forward_preprocess_ex", "dgr_views_forward_preprocess_ex", "dgr_views_mixed_forward_preprocess_ex",
     "dgr_backward_ex", "dgr_views_backward_ex", "dgr_views_mixed_backward_ex",
     "dgr_backward_det_ex", "dgr_views_backward_det_ex", "dgr_views_mixed_backward_det_ex",
-    "dgr_camera_grad_scratch_bytes",
+    "dgr_camera_grad_scratch_bytes", "dgr_densify_plan_ex",
 )
 
 _lib = None
@@ -181,6 +188,9 @@ def load():
     lib.dgr_densify_scratch_bytes.argtypes = [i32]
     lib.dgr_densify_plan.restype = ctypes.c_int
     lib.dgr_densify_plan.argtypes = [i32, vp, vp, vp, vp, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, i32, vp, vp, vp]
+    lib.dgr_densify_plan_ex.restype = ctypes.c_int
+    lib.dgr_densify_plan_ex.argtypes = [i32, vp, vp, vp, vp, vp, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
+                                        ctypes.c_float, i32, vp, vp, vp]
     lib.dgr_densify_apply.restype = ctypes.c_int
     lib.dgr_densify_apply.argtypes = [i32, ctypes.POINTER(DgrDensifyTensors), vp, vp, vp]
     lib.dgr_mark_visible.restype = ctypes.c_int

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "../../include/dgr_b200.h"
+#include "dgr_absgrad.cuh"
 #include "dgr_backward.cuh"
 #include "dgr_binning.cuh"
 #include "dgr_camgrad.cuh"
@@ -172,20 +173,34 @@ static_assert(DGR_RASTER_ANTIALIAS < 256u, "the known flags must fit the flags b
 int raster_flags(const DgrRasterOptions *opt, uint32_t *flags) {
     *flags = opt ? opt->flags : 0u;
     if (*flags & DGR_RASTER_CAMERA_GRADS) return fail(-1, "DgrRasterOptions: DGR_RASTER_CAMERA_GRADS is backward-only (a forward call refuses it)");
+    if (*flags & DGR_RASTER_ABS_GRAD) return fail(-1, "DgrRasterOptions: DGR_RASTER_ABS_GRAD is backward-only (a forward call refuses it)");
     if (*flags & ~DGR_RASTER_ANTIALIAS) return fail(-1, "DgrRasterOptions: unknown flag bits");
     return 0;
 }
-// The backward calls' options: the recorded / compared flags (DGR_RASTER_ANTIALIAS) and, with DGR_RASTER_CAMERA_GRADS, the camera
-// outputs (*cam; NULL without the bit).
-int raster_flags_bwd(const DgrRasterOptions *opt, uint32_t *flags, const DgrCameraGrads **cam) {
+// The backward calls' options: the recorded / compared flags (DGR_RASTER_ANTIALIAS), with DGR_RASTER_CAMERA_GRADS the camera
+// outputs (*cam; NULL without the bit) and with DGR_RASTER_ABS_GRAD the absolute-gradient statistic (*abs_accum; NULL without it).
+int raster_flags_bwd(const DgrRasterOptions *opt, uint32_t *flags, const DgrCameraGrads **cam, float **abs_accum) {
     *flags = opt ? opt->flags : 0u;
     *cam = nullptr;
-    if (*flags & ~(DGR_RASTER_ANTIALIAS | DGR_RASTER_CAMERA_GRADS)) return fail(-1, "DgrRasterOptions: unknown flag bits");
+    *abs_accum = nullptr;
+    if (*flags & ~(DGR_RASTER_ANTIALIAS | DGR_RASTER_CAMERA_GRADS | DGR_RASTER_ABS_GRAD)) return fail(-1, "DgrRasterOptions: unknown flag bits");
     if (*flags & DGR_RASTER_CAMERA_GRADS) {
         if (!opt->camera) return fail(-1, "DgrRasterOptions: DGR_RASTER_CAMERA_GRADS with camera == NULL");
         *cam = opt->camera;
     }
+    if (*flags & DGR_RASTER_ABS_GRAD) {
+        if (!opt->xyz_gradient_accum_abs) return fail(-1, "DgrRasterOptions: DGR_RASTER_ABS_GRAD with xyz_gradient_accum_abs == NULL");
+        *abs_accum = opt->xyz_gradient_accum_abs;
+    }
     *flags &= DGR_RASTER_ANTIALIAS;
+    return 0;
+}
+// DGR_RASTER_ABS_GRAD after the per-Gaussian backward: the statistic of the views in stats_views from moment slots 10 and 11
+int absgrad_stats(int P, int V, const ViewTable &vt, uint64_t stats_views, const int *radii, const float *grad_rec, float *abs_accum,
+                  int debug, cudaStream_t st) {
+    DGR_KERNEL("absgrad_stats", st, debug, launch_k(absgrad_stats_kernel, dim3((unsigned)((P + kAbsStatsThreads - 1) / kAbsStatsThreads)),
+                                                    dim3(kAbsStatsThreads), 0, st, false, P, V, vt, (unsigned long long)stats_views, radii,
+                                                    grad_rec, abs_accum));
     return 0;
 }
 int check_camera(const DgrCameraGrads *cam, int V, int P) {
@@ -462,7 +477,7 @@ int check_det(const DetArgs &d, const DgrGaussianGrads *gout, uint64_t capacity,
 // det_moments_gather, which leaves grad_rec as the default render kernel would, summed in a fixed order.  vt = NULL: single view.
 int det_render(DevInfo *dv, const DetArgs &d, long long R, int H, int W, int gx, const ViewTable *vt, int tiles, const char *image,
                const ImageLayout &IL, char *geom, const GeomLayout &GL, const char *binning, const BinningLayout &BL, bool lazy,
-               const float *bg, const DgrImageGrads *gin, float *grad_rec, int debug, cudaStream_t st) {
+               const float *bg, const DgrImageGrads *gin, float *grad_rec, bool abs, int debug, cudaStream_t st) {
     if (debug) {                                     // debug: the caller's instance count against the forward's own (a host sync)
         unsigned long long n_fwd = 0;
         DGR_CUDA(cudaMemcpyAsync(&n_fwd, geom + offsetof(GeomHeader, n_inst), sizeof(n_fwd), cudaMemcpyDeviceToHost, st));
@@ -508,13 +523,23 @@ int det_render(DevInfo *dv, const DetArgs &d, long long R, int H, int W, int gx,
     };
     int e = 0;
     if (d.instances == 0) {}                         // nothing binned: no instance row to fill (the gather flags any touched record)
+    else if (abs) {
+        if (vt) e = lazy ? launch(render_views_bwd_det_abs_kernel<true>, "render_views_bwd_det_abs", *vt)
+                         : launch(render_views_bwd_det_abs_kernel<false>, "render_views_bwd_det_abs", *vt);
+        else e = lazy ? launch(render_bwd_det_abs_kernel<true>, "render_bwd_det_abs", H, W, gx)
+                      : launch(render_bwd_det_abs_kernel<false>, "render_bwd_det_abs", H, W, gx);
+    }
     else if (vt) e = lazy ? launch(render_views_bwd_det_kernel<true>, "render_views_bwd_det", *vt)
                      : launch(render_views_bwd_det_kernel<false>, "render_views_bwd_det", *vt);
     else e = lazy ? launch(render_bwd_det_kernel<true>, "render_bwd_det", H, W, gx)
                   : launch(render_bwd_det_kernel<false>, "render_bwd_det", H, W, gx);
     if (e) return e;
-    DGR_KERNEL("det_moments_gather", st, debug, launch_k(det_moments_gather_kernel, dim3(nb), dim3(256), 0, st, true, R, touched,
-                                                         (const unsigned *)goff, (const float *)mom, n_slots, grad_rec));
+    if (abs)
+        DGR_KERNEL("det_moments_gather_abs", st, debug, launch_k(det_moments_gather_abs_kernel, dim3(nb), dim3(256), 0, st, true, R, touched,
+                                                                 (const unsigned *)goff, (const float *)mom, n_slots, grad_rec));
+    else
+        DGR_KERNEL("det_moments_gather", st, debug, launch_k(det_moments_gather_kernel, dim3(nb), dim3(256), 0, st, true, R, touched,
+                                                             (const unsigned *)goff, (const float *)mom, n_slots, grad_rec));
     return 0;
 }
 }  // namespace
@@ -706,7 +731,8 @@ static int flat_segs(int32_t n_seg, const int64_t *seg_off, const int32_t *seg_s
 // dgr_backward (det = NULL) and dgr_backward_det
 static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                            int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                           const DgrGaussianGrads *gout, const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, void *stream) {
+                           const DgrGaussianGrads *gout, const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, float *abs_accum,
+                           void *stream) {
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
     if (int e = check_camera(cam, 1, g->P)) return e;
@@ -737,7 +763,7 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
         DevInfo *dv = dev_info();
         if (!dv) return -1;
         if (int e = det_render(dv, *det, g->P, H, W, IL.gx, nullptr, tiles, image, IL, geom, GL, binning, BL, staging == DGR_STAGING_BY_ID,
-                               s->bg, gin, grad_rec, s->debug, st)) return e;
+                               s->bg, gin, grad_rec, abs_accum != nullptr, s->debug, st)) return e;
     } else if (binning && capacity > 0) {
         DevInfo *dv = dev_info();
         if (!dv) return -1;
@@ -763,6 +789,24 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
 #define DGR_RENDER_BWD(PPL_, U_) do { if (lazy) DGR_RENDER_BWD_L(PPL_, U_, true); else DGR_RENDER_BWD_L(PPL_, U_, false); } while (0)
         // the record staging the forward chose (dgr_forward_render): only then does the sorted copy exist
         const bool lazy = staging == DGR_STAGING_BY_ID;
+        if (abs_accum) {                                               // DGR_RASTER_ABS_GRAD: the default shape's ABS variant, whatever the knobs
+            const CostOrder co1 = cost_order(image, IL, tiles, 1);
+            auto launch = [&](auto kernel) -> int {
+                const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;
+                int grid_ = min(persistent_grid(dv, kernel, kRenderThreads, smem_), (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);
+                if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);
+                DGR_KERNEL("render_bwd_abs", st, s->debug,
+                           launch_k(kernel, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, H, W, IL.gx,
+                                    reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co1,
+                                    reinterpret_cast<const uint2 *>(image + IL.off_oranges),
+                                    reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec),
+                                    (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),
+                                    s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),
+                                    reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, grad_rec));
+                return 0;
+            };
+            if (int e = lazy ? launch(render_bwd_abs_kernel<true>) : launch(render_bwd_abs_kernel<false>)) return e;
+        } else
         if (ppl == 1 && ub != 1 && !lazy && !g_rowsum.load()) {       // A/B: the default shape with the per-pixel step 2
 #define DGR_BWD_OLD_ render_bwd_kernel<1, 2, false, false>
             const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;
@@ -785,6 +829,11 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
     }
     const bool aa = flags & DGR_RASTER_ANTIALIAS;
     DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, aa, st));
+    if (abs_accum) {
+        ViewTable vt_abs;                            // one view of H x W
+        memset(&vt_abs, 0, sizeof(vt_abs)); vt_abs.H[0] = H; vt_abs.W[0] = W;
+        if (int e = absgrad_stats(g->P, 1, vt_abs, 1u, radii, grad_rec, abs_accum, s->debug, st)) return e;
+    }
     if (cam)
         return camera_grads(s, g, cam, 1, vt1, make_float2(s->tanfovx, s->tanfovy), nullptr, radii,
                             reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, aa, st);
@@ -796,7 +845,7 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
                  const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_backward");
     (void)out_alpha;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, nullptr, stream);
 }
 
 int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -806,8 +855,9 @@ int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, c
     (void)out_alpha;
     uint32_t flags = 0;
     const DgrCameraGrads *cam = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, stream);
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, abs_accum, stream);
 }
 
 size_t dgr_det_scratch_bytes(uint64_t instances, int64_t records) { return DetLayout(instances, records).total; }
@@ -819,7 +869,7 @@ int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom_v, 
     NvtxRange nvtx_("dgr_backward_det");
     (void)out_alpha;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, nullptr, stream);
 }
 
 int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -830,9 +880,10 @@ int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_
     (void)out_alpha;
     uint32_t flags = 0;
     const DgrCameraGrads *cam = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, abs_accum, stream);
 }
 
 }  // extern "C"
@@ -1056,7 +1107,7 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
 
 int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                    int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, uint64_t stats_views,
-                   const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, void *stream) {
+                   const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, float *abs_accum, void *stream) {
     if (det)
         if (int e = check_det(*det, gout, capacity, (long long)g->P * s->V)) return e;
     if (int e = check_camera(cam, s->V, g->P)) return e;
@@ -1076,7 +1127,7 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
         DevInfo *dv = dev_info();
         if (!dv) return -1;
         if (int e = det_render(dv, *det, (long long)g->P * s->V, 0, 0, 0, &b.vt, tiles, image, IL, geom, GL, binning, BL,
-                               staging == DGR_STAGING_BY_ID, s->bg, gin, grad_rec, s->debug, st)) return e;
+                               staging == DGR_STAGING_BY_ID, s->bg, gin, grad_rec, abs_accum != nullptr, s->debug, st)) return e;
     } else if (binning && capacity > 0) {
         DevInfo *dv = dev_info();
         if (!dv) return -1;
@@ -1084,14 +1135,14 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
         unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
         const CostOrder co = cost_order(image, IL, tiles, 1);
         const bool lazy = staging == DGR_STAGING_BY_ID;
-#define DGR_VIEWS_BWD(L_)                                                                                                       \
+#define DGR_VIEWS_BWD_K(K_, NAME_)                                                                                              \
     do {                                                                                                                       \
         const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;                                                                \
-        int grid_ = min(persistent_grid(dv, render_views_bwd_kernel<L_>, kRenderThreads, smem_),                               \
+        int grid_ = min(persistent_grid(dv, K_, kRenderThreads, smem_),                                                        \
                         (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);                                     \
         if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);                                              \
-        DGR_KERNEL("render_views_bwd", st, s->debug,                                                                           \
-                   launch_k(render_views_bwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, b.vt,    \
+        DGR_KERNEL(NAME_, st, s->debug,                                                                                        \
+                   launch_k(K_, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, b.vt,                           \
                             reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co, \
                             reinterpret_cast<const uint2 *>(image + IL.off_oranges),                                           \
                             reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec), \
@@ -1100,13 +1151,21 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
                             reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, \
                             grad_rec));                                                                                        \
     } while (0)
-        if (lazy) DGR_VIEWS_BWD(true); else DGR_VIEWS_BWD(false);
-#undef DGR_VIEWS_BWD
+        if (abs_accum) {                             // DGR_RASTER_ABS_GRAD: the ABS variant of the same kernel
+            if (lazy) DGR_VIEWS_BWD_K(render_views_bwd_abs_kernel<true>, "render_views_bwd_abs");
+            else DGR_VIEWS_BWD_K(render_views_bwd_abs_kernel<false>, "render_views_bwd_abs");
+        } else {
+            if (lazy) DGR_VIEWS_BWD_K(render_views_bwd_kernel<true>, "render_views_bwd");
+            else DGR_VIEWS_BWD_K(render_views_bwd_kernel<false>, "render_views_bwd");
+        }
+#undef DGR_VIEWS_BWD_K
     }
     const bool aa = flags & DGR_RASTER_ANTIALIAS;
     DGR_KERNEL("preprocess_views_bwd", st, s->debug,
                DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, b, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout,
                                   stats_views, aa, st));
+    if (abs_accum)
+        if (int e = absgrad_stats(g->P, s->V, b.vt, stats_views, radii, grad_rec, abs_accum, s->debug, st)) return e;
     if (cam)
         return camera_grads(s, g, cam, s->V, b.vt, make_float2(0.f, 0.f), s->tanfov, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched),
                             grad_rec, aa, st);
@@ -1149,7 +1208,7 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
 
 static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                                const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
-                               const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, void *stream) {
+                               const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, const float *abs_accum, void *stream) {
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1157,15 +1216,17 @@ static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *g
         return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
     if (gout->xyz_gradient_accum || gout->denom || gout->max_radii2D)
         return fail(-2, "views: the fused densification statistics are not supported by the batched call");
+    if (abs_accum)
+        return fail(-2, "views: DGR_RASTER_ABS_GRAD is not supported by the same-size batched call (it has no densification statistics)");
     if (int e = check_views_grads(gout)) return e;
     return views_backward(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, 0, det, flags,
-                          cam, stream);
+                          cam, nullptr, stream);
 }
 
 int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                        const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_views_backward");
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, nullptr, stream);
 }
 
 int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1174,8 +1235,9 @@ int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v
     NvtxRange nvtx_("dgr_views_backward_ex");
     uint32_t flags = 0;
     const DgrCameraGrads *cam = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, stream);
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, abs_accum, stream);
 }
 
 int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1183,7 +1245,7 @@ int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_
                            void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, nullptr, stream);
 }
 
 int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1192,9 +1254,10 @@ int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *ge
     NvtxRange nvtx_("dgr_views_backward_det_ex");
     uint32_t flags = 0;
     const DgrCameraGrads *cam = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, abs_accum, stream);
 }
 
 // ---- views of different sizes: image_hw = [V,2] (height, width) on the host ------------------------------------------------------
@@ -1243,21 +1306,22 @@ int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, c
 static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
                                 uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
                                 const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, uint32_t flags,
-                                const DgrCameraGrads *cam, void *stream) {
+                                const DgrCameraGrads *cam, float *abs_accum, void *stream) {
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
     if (staging != DGR_STAGING_SORTED && staging != DGR_STAGING_BY_ID)
         return fail(-1, "staging must be DGR_STAGING_SORTED or DGR_STAGING_BY_ID (counts_host[3] of the forward)");
     if (s->V < 64 && (stats_views >> s->V) != 0) return fail(-1, "views mixed: stats_views has a bit at or above V");
-    const bool any_stat = gout->xyz_gradient_accum || gout->denom || gout->max_radii2D;
+    if (abs_accum && !stats_views) return fail(-1, "views mixed: DGR_RASTER_ABS_GRAD with stats_views == 0 (no view to take the statistic from)");
+    const bool any_stat = gout->xyz_gradient_accum || gout->denom || gout->max_radii2D || abs_accum;
     if (stats_views && !any_stat)
         return fail(-1, "views mixed: stats_views is non-zero but no densification statistic buffer is set");
     if (!stats_views && any_stat)
         return fail(-1, "views mixed: a densification statistic buffer is set but stats_views is 0");
     if (int e = check_views_grads(gout)) return e;
     return views_backward(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout,
-                          stats_views, det, flags, cam, stream);
+                          stats_views, det, flags, cam, abs_accum, stream);
 }
 
 int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1265,7 +1329,7 @@ int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const D
                              const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward");
     return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, 0u,
-                                nullptr, stream);
+                                nullptr, nullptr, stream);
 }
 
 int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1274,9 +1338,10 @@ int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, cons
     NvtxRange nvtx_("dgr_views_mixed_backward_ex");
     uint32_t flags = 0;
     const DgrCameraGrads *cam = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, flags,
-                                cam, stream);
+                                cam, abs_accum, stream);
 }
 
 int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1285,7 +1350,8 @@ int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, con
                                  uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, 0u, nullptr, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, 0u, nullptr,
+                                nullptr, stream);
 }
 
 int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1295,10 +1361,11 @@ int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, 
     NvtxRange nvtx_("dgr_views_mixed_backward_det_ex");
     uint32_t flags = 0;
     const DgrCameraGrads *cam = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam)) return e;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
     return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, flags,
-                                cam, stream);
+                                cam, abs_accum, stream);
 }
 
 }  // extern "C"
@@ -1431,6 +1498,32 @@ int dgr_densify_plan(int32_t P, const float *xyz_gradient_accum, const float *de
         DGR_KERNEL("densify_classify", st, 0,
                    densify_classify_kernel<<<L.nblk, kDensifyThreads, 0, st>>>(P, xyz_gradient_accum, denom, opacity_raw, scaling_raw, prm,
                                                                                 reinterpret_cast<unsigned char *>(scratch + L.off_class), counts));
+    else
+        DGR_CUDA(cudaMemsetAsync(counts, 0, 16, st));
+    DGR_KERNEL("densify_offsets", st, 0, densify_offsets_kernel<<<1, 1024, 0, st>>>(P > 0 ? L.nblk : 1, counts, offsets, totals));
+    if (counts_host) DGR_CUDA(cudaMemcpyAsync(counts_host, totals, 4 * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    return 0;
+}
+
+int dgr_densify_plan_ex(int32_t P, const float *xyz_gradient_accum, const float *xyz_gradient_accum_abs, const float *denom,
+                        const float *opacity_raw, const float *scaling_raw, float grad_threshold, float abs_grad_threshold,
+                        float dense_extent, float min_opacity, float max_world, int32_t use_world, void *scratch_v,
+                        uint32_t *counts_host, void *stream) {
+    NvtxRange nvtx_("dgr_densify_plan_ex");
+    if (P < 0) return fail(-1, "P < 0");
+    if (!scratch_v || (P > 0 && (!xyz_gradient_accum || !xyz_gradient_accum_abs || !denom || !opacity_raw || !scaling_raw)))
+        return fail(-1, "NULL argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *scratch = (char *)scratch_v;
+    DensifyLayout L(P);
+    unsigned *counts = reinterpret_cast<unsigned *>(scratch + L.off_counts), *offsets = reinterpret_cast<unsigned *>(scratch + L.off_offsets);
+    unsigned *totals = reinterpret_cast<unsigned *>(scratch + L.off_totals);
+    DensifyParams prm{grad_threshold, dense_extent, min_opacity, max_world, use_world};
+    if (P > 0)
+        DGR_KERNEL("densify_classify_abs", st, 0,
+                   densify_classify_abs_kernel<<<L.nblk, kDensifyThreads, 0, st>>>(P, xyz_gradient_accum, xyz_gradient_accum_abs, denom, opacity_raw,
+                                                                                    scaling_raw, prm, abs_grad_threshold,
+                                                                                    reinterpret_cast<unsigned char *>(scratch + L.off_class), counts));
     else
         DGR_CUDA(cudaMemsetAsync(counts, 0, 16, st));
     DGR_KERNEL("densify_offsets", st, 0, densify_offsets_kernel<<<1, 1024, 0, st>>>(P > 0 ? L.nblk : 1, counts, offsets, totals));

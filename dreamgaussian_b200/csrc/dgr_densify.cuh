@@ -53,14 +53,23 @@ struct DensifyLayout {
     }
 };
 
+// ABS (dgr_densify_plan_ex): AbsGS's rule (Ye et al., 2024) — clone by the default statistic as above, split by the absolute one,
+// accum_abs / denom >= abs_threshold (NaN -> 0 likewise).
+template <bool ABS = false>
 __device__ __forceinline__ unsigned densify_class(int i, const float *accum, const float *denom, const float *opacity_raw,
-                                                  const float *scaling_raw, const DensifyParams &prm) {
+                                                  const float *scaling_raw, const DensifyParams &prm, const float *accum_abs = nullptr,
+                                                  float abs_threshold = 0.f) {
     float g = accum[i] / denom[i];                         // grads = xyz_gradient_accum / denom; grads[isnan] = 0 (:593-594)
     if (g != g) g = 0.f;
     const float s0 = expf(scaling_raw[3 * i]), s1 = expf(scaling_raw[3 * i + 1]), s2 = expf(scaling_raw[3 * i + 2]);
     const float smax = fmaxf(s0, fmaxf(s1, s2));
     const bool clone = (fabsf(g) >= prm.grad_threshold) && (smax <= prm.dense_extent);           // :583-585
-    const bool split = (g >= prm.grad_threshold) && (smax > prm.dense_extent);                   // :558-562
+    bool split = (g >= prm.grad_threshold) && (smax > prm.dense_extent);                         // :558-562
+    if constexpr (ABS) {
+        float ga = accum_abs[i] / denom[i];
+        if (ga != ga) ga = 0.f;
+        split = (ga >= abs_threshold) && (smax > prm.dense_extent);
+    }
     const float o = 1.f / (1.f + expf(-opacity_raw[i]));
     const bool low = o < prm.min_opacity;                                                        // :601
     const bool prune_self = low || (prm.use_world && smax > prm.max_world);                      // :602-605 (max_radii2D was just zeroed: never)
@@ -85,6 +94,25 @@ densify_classify_kernel(int P, const float *__restrict__ accum, const float *__r
     const int i = blockIdx.x * kDensifyThreads + threadIdx.x;
     unsigned c = 0;
     if (i < P) { c = densify_class(i, accum, denom, opacity_raw, scaling_raw, prm); cls[i] = (unsigned char)c; }
+#pragma unroll
+    for (int b = 0; b < 4; b++) {
+        const unsigned m = __ballot_sync(0xffffffffu, (c >> b) & 1u);
+        if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s_cnt[b], (unsigned)__popc(m));
+    }
+    __syncthreads();
+    if (threadIdx.x < 4) block_counts[blockIdx.x * 4 + threadIdx.x] = s_cnt[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(kDensifyThreads)
+densify_classify_abs_kernel(int P, const float *__restrict__ accum, const float *__restrict__ accum_abs, const float *__restrict__ denom,
+                            const float *__restrict__ opacity_raw, const float *__restrict__ scaling_raw, DensifyParams prm,
+                            float abs_threshold, unsigned char *__restrict__ cls, unsigned *__restrict__ block_counts) {
+    __shared__ unsigned s_cnt[4];
+    if (threadIdx.x < 4) s_cnt[threadIdx.x] = 0u;
+    __syncthreads();
+    const int i = blockIdx.x * kDensifyThreads + threadIdx.x;
+    unsigned c = 0;
+    if (i < P) { c = densify_class<true>(i, accum, denom, opacity_raw, scaling_raw, prm, accum_abs, abs_threshold); cls[i] = (unsigned char)c; }
 #pragma unroll
     for (int b = 0; b < 4; b++) {
         const unsigned m = __ballot_sync(0xffffffffu, (c >> b) & 1u);

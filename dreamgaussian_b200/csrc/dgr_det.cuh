@@ -54,7 +54,8 @@ __global__ void __launch_bounds__(256) det_counts_kernel(long long R, const unsi
     if (r < R) counts[r] = __ldg(touched + r) & kTouchedMask;
 }
 
-template <bool LAZY, bool VIEWS>
+// ABS (DGR_RASTER_ABS_GRAD): step 2 also leaves the absolute moments of render_bwd_body<.., ABS> in floats 10 and 11 of each row.
+template <bool LAZY, bool VIEWS, bool ABS = false>
 __device__ __forceinline__ void
 render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
                     const unsigned *__restrict__ n_tiles_nonempty, unsigned long long *__restrict__ work_next,
@@ -154,6 +155,7 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
 
         int nslots = 0, cap_j = 0;                                   // parked records: lane L < kBatch owns slot L
         float cap_cx = 0.f, cap_cy = 0.f;
+        float cap_ca = 0.f, cap_cb = 0.f, cap_cc = 0.f;              // ABS: the record's conic (A, B, C)
         auto flush = [&](int buf) {                                  // step 2 of the default kernel (per-row form), to shared memory
             __syncwarp();
             const float ccx = __shfl_sync(0xffffffffu, cap_cx, my_r), ccy = __shfl_sync(0xffffffffu, cap_cy, my_r);
@@ -161,6 +163,12 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
             const int kb = my_q * kPixPerLane;
             const float dy = ccy - (float)my_q;
             float s0 = 0.f, s1 = 0.f, s3 = 0.f, v6 = 0.f, v7 = 0.f, v8 = 0.f, v9 = 0.f;
+            float v10 = 0.f, v11 = 0.f, ca = 0.f, cb = 0.f, bdy = 0.f, cdy = 0.f;
+            if constexpr (ABS) {
+                ca = __shfl_sync(0xffffffffu, cap_ca, my_r); cb = __shfl_sync(0xffffffffu, cap_cb, my_r);
+                const float cc = __shfl_sync(0xffffffffu, cap_cc, my_r);
+                bdy = cb * dy; cdy = cc * dy;
+            }
 #pragma unroll
             for (int i = 0; i < 8; i += 2) {
                 const float4 t = *reinterpret_cast<const float4 *>(row + 2 * (kb + i));
@@ -172,6 +180,11 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
                     const float udx = u * dx;
                     s0 += u; s1 += udx; s3 = __fmaf_rn(udx, dx, s3);
                     v6 = __fmaf_rn(w, g.x, v6); v7 = __fmaf_rn(w, g.y, v7); v8 = __fmaf_rn(w, g.z, v8); v9 = __fmaf_rn(w, g.w, v9);
+                    if constexpr (ABS) {
+                        const float au = fabsf(u);
+                        v10 = __fmaf_rn(au, fabsf(__fmaf_rn(ca, dx, bdy)), v10);
+                        v11 = __fmaf_rn(au, fabsf(__fmaf_rn(cb, dx, cdy)), v11);
+                    }
                 }
             }
             float v0 = s0, v1 = s1, v3 = s3, v2 = dy * s0, v4 = dy * s1, v5 = (dy * dy) * s0;
@@ -182,10 +195,11 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
                 v4 += __shfl_xor_sync(0xffffffffu, v4, o); v5 += __shfl_xor_sync(0xffffffffu, v5, o);
                 v6 += __shfl_xor_sync(0xffffffffu, v6, o); v7 += __shfl_xor_sync(0xffffffffu, v7, o);
                 v8 += __shfl_xor_sync(0xffffffffu, v8, o); v9 += __shfl_xor_sync(0xffffffffu, v9, o);
+                if constexpr (ABS) { v10 += __shfl_xor_sync(0xffffffffu, v10, o); v11 += __shfl_xor_sync(0xffffffffu, v11, o); }
             }
             if (lane < nslots) {
                 float4 *dst = sm.mom[buf][warp][cap_j];
-                dst[0] = make_float4(v0, v1, v2, v3); dst[1] = make_float4(v4, v5, v6, v7); dst[2] = make_float4(v8, v9, 0.f, 0.f);
+                dst[0] = make_float4(v0, v1, v2, v3); dst[1] = make_float4(v4, v5, v6, v7); dst[2] = make_float4(v8, v9, v10, v11);
             }
             nslots = 0;
             __syncwarp();
@@ -209,7 +223,7 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
                     js[u] = 0;
                     if (mask) { js[u] = bfind_u32(mask); mask &= ~(1u << js[u]); nh = u + 1; }      // last record of the chunk first
                 }
-                float agv[U], av[U], rcx[U], rcy[U], dep[U], cr[U], cg[U], cb[U];
+                float agv[U], av[U], rcx[U], rcy[U], dep[U], cr[U], cg[U], cb[U], rqa[U], rqb[U], rqc[U];
                 bool okv[U], any_ok[U];
 #pragma unroll
                 for (int u = 0; u < U; u++) {
@@ -219,6 +233,7 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
                         const float4 q0 = r->q0, q1 = r->q1, q2 = r->q2;
                         const unsigned gidx = (unsigned)(c * kChunk + js[u]);
                         rcx[u] = q0.x - (float)wx0; rcy[u] = q0.y - (float)wy0; dep[u] = q1.z; cr[u] = q2.x; cg[u] = q2.y; cb[u] = q2.z;
+                        if constexpr (ABS) { rqa[u] = q0.z; rqb[u] = q0.w; rqc[u] = q1.x; }
                         const float dx = q0.x - fx, dy = q0.y - fy;
                         const float p2 = eval_power2(q0, q1, dx, dy);
                         agv[u] = __fmul_rn(q1.y, ex2_approx(p2));
@@ -241,7 +256,10 @@ render_bwd_det_body(int H, int W, int gx, const unsigned *__restrict__ tile_orde
                             uu = agv[u] * dL_da;
                         }
                         *reinterpret_cast<float2 *>(&sm.uw[warp][nslots][2 * lane]) = make_float2(uu, w);
-                        if (lane == nslots) { cap_cx = rcx[u]; cap_cy = rcy[u]; cap_j = js[u]; }
+                        if (lane == nslots) {
+                            cap_cx = rcx[u]; cap_cy = rcy[u]; cap_j = js[u];
+                            if constexpr (ABS) { cap_ca = rqa[u] * (-2.f / kLog2e); cap_cb = rqb[u] * (-1.f / kLog2e); cap_cc = rqc[u] * (-2.f / kLog2e); }
+                        }
                         nslots++;
                         if (nslots == kBatch) flush(buf);
                     }
@@ -303,12 +321,39 @@ render_views_bwd_det_kernel(const __grid_constant__ ViewTable vt, const unsigned
                                     n_slots, bg, final_T, n_contrib, gC, gD, gA, det_mom, &vt);
 }
 
+// DGR_RASTER_ABS_GRAD: the same two kernels with the absolute moments (separate kernels: the ones above stay as they were)
+template <bool LAZY>
+__global__ void __launch_bounds__(kDetThreads)
+render_bwd_det_abs_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+                          const unsigned *__restrict__ n_tiles_nonempty, unsigned long long *__restrict__ work_next,
+                          const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
+                          const unsigned *__restrict__ goff, unsigned long long n_slots, const float *__restrict__ bg,
+                          const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
+                          const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA, float *__restrict__ det_mom) {
+    render_bwd_det_body<LAZY, false, true>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, work_next, rec_sorted, rec, ids_sorted, goff,
+                                           n_slots, bg, final_T, n_contrib, gC, gD, gA, det_mom, nullptr);
+}
+
+template <bool LAZY>
+__global__ void __launch_bounds__(kDetThreads)
+render_views_bwd_det_abs_kernel(const __grid_constant__ ViewTable vt, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+                                const unsigned *__restrict__ n_tiles_nonempty, unsigned long long *__restrict__ work_next,
+                                const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
+                                const unsigned *__restrict__ goff, unsigned long long n_slots, const float *__restrict__ bg,
+                                const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
+                                const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA, float *__restrict__ det_mom) {
+    render_bwd_det_body<LAZY, true, true>(0, 0, 0, tile_order, order_ranges, n_tiles_nonempty, work_next, rec_sorted, rec, ids_sorted, goff,
+                                          n_slots, bg, final_T, n_contrib, gC, gD, gA, det_mom, &vt);
+}
+
 // One thread per record: the moments of its instance slots, summed in slot order (the row-major order of its tiles) -> grad_rec.
 // Records that touch no tile keep the zero row of the backward's memset.  A record whose slots run past n_slots (the caller passed
 // fewer instances than the forward binned) gets a NaN row: its gradients come out visibly wrong instead of silently short.
-__global__ void __launch_bounds__(256)
-det_moments_gather_kernel(long long R, const unsigned *__restrict__ touched, const unsigned *__restrict__ goff,
-                          const float *__restrict__ det_mom, unsigned long long n_slots, float *__restrict__ grad_rec) {
+// ABS: also the absolute moments (floats 10 and 11).
+template <bool ABS>
+__device__ __forceinline__ void
+det_moments_gather_body(long long R, const unsigned *__restrict__ touched, const unsigned *__restrict__ goff,
+                        const float *__restrict__ det_mom, unsigned long long n_slots, float *__restrict__ grad_rec) {
     pdl_trigger();
     pdl_wait();                          // the instance moments of render_bwd_det
     const long long r = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -319,7 +364,7 @@ det_moments_gather_kernel(long long R, const unsigned *__restrict__ touched, con
     float4 *dst = reinterpret_cast<float4 *>(grad_rec + (size_t)r * kGradRecFloats);
     if (o + t > n_slots) {
         const float nan = __int_as_float(0x7fffffff);
-        dst[0] = make_float4(nan, nan, nan, nan); dst[1] = dst[0]; dst[2] = make_float4(nan, nan, 0.f, 0.f);
+        dst[0] = make_float4(nan, nan, nan, nan); dst[1] = dst[0]; dst[2] = make_float4(nan, nan, ABS ? nan : 0.f, ABS ? nan : 0.f);
         return;
     }
     float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a, c = a;
@@ -329,8 +374,21 @@ det_moments_gather_kernel(long long R, const unsigned *__restrict__ touched, con
         a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
         b.x += y.x; b.y += y.y; b.z += y.z; b.w += y.w;
         c.x += z.x; c.y += z.y;
+        if constexpr (ABS) { c.z += z.z; c.w += z.w; }
     }
     dst[0] = a; dst[1] = b; dst[2] = c;
+}
+
+__global__ void __launch_bounds__(256)
+det_moments_gather_kernel(long long R, const unsigned *__restrict__ touched, const unsigned *__restrict__ goff,
+                          const float *__restrict__ det_mom, unsigned long long n_slots, float *__restrict__ grad_rec) {
+    det_moments_gather_body<false>(R, touched, goff, det_mom, n_slots, grad_rec);
+}
+
+__global__ void __launch_bounds__(256)
+det_moments_gather_abs_kernel(long long R, const unsigned *__restrict__ touched, const unsigned *__restrict__ goff,
+                              const float *__restrict__ det_mom, unsigned long long n_slots, float *__restrict__ grad_rec) {
+    det_moments_gather_body<true>(R, touched, goff, det_mom, n_slots, grad_rec);
 }
 
 }  // namespace dgr

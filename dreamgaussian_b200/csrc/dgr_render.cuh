@@ -435,7 +435,10 @@ struct BwdSmem {
 // instructions per (record, pixel) on the u side).  ROWSUM = false keeps the per-pixel form (A/B: dgr_set_tuning bit 26).
 // VIEWS: the batched backward (dgr_views_backward), tiles and images numbered as in render_fwd_body; the moments go to the
 // records of the batch (the ids the sort wrote are record numbers v P + g).
-template <int PPL, int U, bool LAZY, bool ROWSUM, bool VIEWS>
+// ABS (DGR_RASTER_ABS_GRAD, per-row step 2 only): step 2 also sums |u (A dx + B dy)| and |u (B dx + C dy)| over the pixels, the
+// per-pixel terms of the pixel-space mean gradient before they can cancel, into moment slots 10 and 11 (absgrad_stats_kernel
+// turns them into the AbsGS statistic).  The conic is parked with the record, its -1/2 log2 e scaling undone once per record.
+template <int PPL, int U, bool LAZY, bool ROWSUM, bool VIEWS, bool ABS = false>
 __device__ __forceinline__ void
 render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
                   unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
@@ -444,6 +447,7 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                   const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
                   const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
                   float *__restrict__ grad_rec, const ViewTable *vt) {
+    static_assert(!ABS || ROWSUM, "the absolute moments exist in the per-row step 2 only");
     using ST = SubTile<PPL>;
     using SM = BwdSmem<PPL>;
     constexpr int kPix = SM::kPix;
@@ -555,12 +559,17 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
         int nslots = 0;
         float cap_cx = 0.f, cap_cy = 0.f;
         unsigned cap_id = 0;
+        float cap_ca = 0.f, cap_cb = 0.f, cap_cc = 0.f;          // ABS: the record's conic (A, B, C)
 
         // step 2: the kBatch parked records -> 10 moments each.  Lane (my_r, my_q) covers pixel group my_q of record my_r.
         auto flush = [&]() {
             __syncwarp();
             const float ccx = __shfl_sync(0xffffffffu, cap_cx, my_r), ccy = __shfl_sync(0xffffffffu, cap_cy, my_r);
             float v0 = 0.f, v1 = 0.f, v2 = 0.f, v3 = 0.f, v4 = 0.f, v5 = 0.f, v6 = 0.f, v7 = 0.f, v8 = 0.f, v9 = 0.f;
+            float v10 = 0.f, v11 = 0.f, ca = 0.f, cb = 0.f, cc = 0.f;
+            if constexpr (ABS) {
+                ca = __shfl_sync(0xffffffffu, cap_ca, my_r); cb = __shfl_sync(0xffffffffu, cap_cb, my_r); cc = __shfl_sync(0xffffffffu, cap_cc, my_r);
+            }
             const float *row = &sm.uw[my_r][0];
             if (ROWSUM) {
                 static_assert(kPixPerLane % 8 == 0, "a lane's pixels come in rows of 8");
@@ -571,6 +580,7 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                     const float dxb = ccx - (float)((PPL == 4 && (pp & 1)) ? 8 : 0);
                     const float dy = ccy - (float)((pl >> 3) + ((PPL == 4) ? (pp >> 1) * 4 : pp * 4));
                     float s0 = 0.f, s1 = 0.f, s3 = 0.f;
+                    const float bdy = ABS ? cb * dy : 0.f, cdy = ABS ? cc * dy : 0.f;   // ABS: the row's dy terms of A dx + B dy, B dx + C dy
 #pragma unroll
                     for (int i = 0; i < 8; i += 2) {
                         const float4 t = *reinterpret_cast<const float4 *>(row + 2 * (kb + i));   // (u, w) of pixels kb + i, kb + i + 1
@@ -582,6 +592,11 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                             const float udx = u * dx;
                             s0 += u; s1 += udx; s3 = __fmaf_rn(udx, dx, s3);
                             v6 = __fmaf_rn(w, g.x, v6); v7 = __fmaf_rn(w, g.y, v7); v8 = __fmaf_rn(w, g.z, v8); v9 = __fmaf_rn(w, g.w, v9);
+                            if constexpr (ABS) {
+                                const float au = fabsf(u);
+                                v10 = __fmaf_rn(au, fabsf(__fmaf_rn(ca, dx, bdy)), v10);
+                                v11 = __fmaf_rn(au, fabsf(__fmaf_rn(cb, dx, cdy)), v11);
+                            }
                         }
                     }
                     if (g8 == 0) { v0 = s0; v1 = s1; v3 = s3; v2 = dy * s0; v4 = dy * s1; v5 = (dy * dy) * s0; }
@@ -617,12 +632,14 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                 v4 += __shfl_xor_sync(0xffffffffu, v4, o); v5 += __shfl_xor_sync(0xffffffffu, v5, o);
                 v6 += __shfl_xor_sync(0xffffffffu, v6, o); v7 += __shfl_xor_sync(0xffffffffu, v7, o);
                 v8 += __shfl_xor_sync(0xffffffffu, v8, o); v9 += __shfl_xor_sync(0xffffffffu, v9, o);
+                if constexpr (ABS) { v10 += __shfl_xor_sync(0xffffffffu, v10, o); v11 += __shfl_xor_sync(0xffffffffu, v11, o); }
             }
             if (lane < nslots) {
                 float *dst = grad_rec + (size_t)cap_id * kGradRecFloats;
                 red_add_f32(dst, v0); red_add_f32(dst + 1, v1); red_add_f32(dst + 2, v2); red_add_f32(dst + 3, v3);
                 red_add_f32(dst + 4, v4); red_add_f32(dst + 5, v5); red_add_f32(dst + 6, v6); red_add_f32(dst + 7, v7);
                 red_add_f32(dst + 8, v8); red_add_f32(dst + 9, v9);
+                if constexpr (ABS) { red_add_f32(dst + 10, v10); red_add_f32(dst + 11, v11); }
             }
             nslots = 0;
             __syncwarp();
@@ -646,7 +663,7 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                     js[u] = 0;
                     if (mask) { js[u] = bfind_u32(mask); mask &= ~(1u << js[u]); nh = u + 1; }      // last record of the chunk first
                 }
-                float agv[U][PPL], av[U][PPL], rcx[U], rcy[U], dep[U], cr[U], cg[U], cb[U];
+                float agv[U][PPL], av[U][PPL], rcx[U], rcy[U], dep[U], cr[U], cg[U], cb[U], rqa[U], rqb[U], rqc[U];
                 bool okv[U][PPL], any_ok[U];
 #pragma unroll
                 for (int u = 0; u < U; u++) {
@@ -656,6 +673,7 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                         const float4 q0 = r->q0, q1 = r->q1, q2 = r->q2;
                         const unsigned gidx = (unsigned)(c * kChunk + js[u]);
                         rcx[u] = q0.x - (float)wx0; rcy[u] = q0.y - (float)wy0; dep[u] = q1.z; cr[u] = q2.x; cg[u] = q2.y; cb[u] = q2.z;
+                        if constexpr (ABS) { rqa[u] = q0.z; rqb[u] = q0.w; rqc[u] = q1.x; }
                         bool mine = false;
 #pragma unroll
                         for (int p = 0; p < PPL; p++) {
@@ -688,7 +706,10 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                             *reinterpret_cast<float2 *>(row + 2 * (p * 32 + lane)) = make_float2(uu, w);
                         }
                         const unsigned id_j = __shfl_sync(0xffffffffu, my_id, js[u]);
-                        if (lane == nslots) { cap_cx = rcx[u]; cap_cy = rcy[u]; cap_id = id_j; }
+                        if (lane == nslots) {
+                            cap_cx = rcx[u]; cap_cy = rcy[u]; cap_id = id_j;
+                            if constexpr (ABS) { cap_ca = rqa[u] * (-2.f / kLog2e); cap_cb = rqb[u] * (-1.f / kLog2e); cap_cc = rqc[u] * (-2.f / kLog2e); }
+                        }
                         nslots++;
                         if (nslots == kBatch) flush();
                     }
@@ -730,6 +751,32 @@ render_views_bwd_kernel(const __grid_constant__ ViewTable vt, const unsigned *__
                   const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
                   float *__restrict__ grad_rec) {
     render_bwd_body<1, 2, LAZY, true, true>(0, 0, 0, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, &vt);
+}
+
+// DGR_RASTER_ABS_GRAD: the default shape <1,2> with the per-row step 2 that also leaves the absolute moments in slots 10 and 11
+// (single view and batched).  Separate kernels, so every instantiation above stays as it was.
+template <bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads)
+render_bwd_abs_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
+                  unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ lazy_note,
+                  const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
+                  const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
+                  const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
+                  float *__restrict__ grad_rec) {
+    render_bwd_body<1, 2, LAZY, true, false, true>(H, W, gx, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, nullptr);
+}
+
+template <bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads)
+render_views_bwd_abs_kernel(const __grid_constant__ ViewTable vt, const unsigned *__restrict__ tile_order, const unsigned *__restrict__ n_tiles_nonempty,
+                  unsigned long long *__restrict__ work_next, int two_ended, int sms, CostOrder co, const uint2 *__restrict__ order_ranges,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ lazy_note,
+                  const unsigned *__restrict__ ids_sorted, const float *__restrict__ bg,
+                  const float *__restrict__ final_T, const unsigned *__restrict__ n_contrib,
+                  const float *__restrict__ gC, const float *__restrict__ gD, const float *__restrict__ gA,
+                  float *__restrict__ grad_rec) {
+    render_bwd_body<1, 2, LAZY, true, true, true>(0, 0, 0, tile_order, n_tiles_nonempty, work_next, two_ended, sms, co, order_ranges, rec_sorted, rec, lazy_note, ids_sorted, bg, final_T, n_contrib, gC, gD, gA, grad_rec, &vt);
 }
 
 }  // namespace dgr

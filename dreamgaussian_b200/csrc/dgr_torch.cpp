@@ -174,10 +174,17 @@ forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modif
 
 // Camera gradients (DGR_RASTER_CAMERA_GRADS): appends dL/dviewmatrix, dL/dprojmatrix ([V,16] each, [16] for V = 0: single view)
 // and dL/dcampos ([V,3] / [3]) to g and returns the options of the backward call; without camera, the forward's options unchanged.
-struct CameraOut { DgrCameraGrads cg{}; DgrRasterOptions opt{0u, nullptr}; Tensor scratch; };
+// absgrad (xyz_gradient_accum_abs [P]): DGR_RASTER_ABS_GRAD with it.
+struct CameraOut { DgrCameraGrads cg{}; DgrRasterOptions opt{0u, nullptr, nullptr}; Tensor scratch; };
 void camera_out(bool camera, int64_t V, int64_t P, const DgrRasterOptions &fwd, const torch::TensorOptions &f32, std::vector<Tensor> &g,
-                CameraOut &c) {
+                CameraOut &c, const OptTensor &absgrad) {
     c.opt = fwd;
+    if (float *a = fptr_mut(absgrad)) {
+        TORCH_CHECK_VALUE(absgrad->is_cuda() && absgrad->scalar_type() == torch::kFloat32 && absgrad->is_contiguous() && absgrad->numel() == P,
+                          "xyz_gradient_accum_abs must be a contiguous float32 CUDA tensor of num_points elements");
+        c.opt.flags |= DGR_RASTER_ABS_GRAD;
+        c.opt.xyz_gradient_accum_abs = a;
+    }
     if (!camera) return;
     const std::vector<int64_t> s16 = V ? std::vector<int64_t>{V, 16} : std::vector<int64_t>{16};
     const std::vector<int64_t> s3 = V ? std::vector<int64_t>{V, 3} : std::vector<int64_t>{3};
@@ -194,7 +201,7 @@ void camera_out(bool camera, int64_t V, int64_t P, const DgrRasterOptions &fwd, 
 // camera: + (dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3])
 std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA, bool accumulate,
                              const std::vector<OptTensor> &out, const OptTensor &xyz_gradient_accum, const OptTensor &denom,
-                             const OptTensor &max_radii2D, int64_t push_addr, bool camera) {
+                             const OptTensor &max_radii2D, int64_t push_addr, bool camera, const OptTensor &absgrad) {
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     const int64_t P = st->g.P, M = st->g.M;
     const auto f32 = st->means3D.options();
@@ -219,7 +226,7 @@ std::vector<Tensor> backward(const std::shared_ptr<State> &st, const OptTensor &
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D),
                           reinterpret_cast<const DgrPeerPush *>(push_addr)};      // host struct kept alive by the caller (0 = none)
     CameraOut cam;
-    camera_out(camera, 0, P, st->opt, f32, g, cam);
+    camera_out(camera, 0, P, st->opt, f32, g, cam, absgrad);
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
     if (at::globalContext().deterministicAlgorithms()) {
         Tensor det = det_scratch(st->n_inst, P, f32);
@@ -415,7 +422,8 @@ views_mixed_forward(const std::vector<int32_t> &image_hw, double scale_modifier,
 // dL/dprojmatrix [V,16], dL/dcampos [V,3]).
 std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
                                         bool accumulate, const std::vector<OptTensor> &out, const OptTensor &xyz_gradient_accum,
-                                        const OptTensor &denom, const OptTensor &max_radii2D, uint64_t stats_views, bool camera) {
+                                        const OptTensor &denom, const OptTensor &max_radii2D, uint64_t stats_views, bool camera,
+                                        const OptTensor &absgrad) {
     const c10::cuda::CUDAGuard guard(st->means3D.device());
     const int64_t P = st->g.P, M = st->g.M, V = st->s.V;
     const auto f32 = st->means3D.options();
@@ -435,7 +443,7 @@ std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, c
     DgrGaussianGrads gout{gp(0), gp(1), gp(2), nullptr, gp(3), gp(4), gp(5), nullptr, accumulate ? 1 : 0, gp(6),
                           fptr_mut(xyz_gradient_accum), fptr_mut(denom), fptr_mut(max_radii2D), nullptr};
     CameraOut cam;
-    camera_out(camera, V, P, st->opt, f32, g, cam);
+    camera_out(camera, V, P, st->opt, f32, g, cam, absgrad);
     void *stream = c10::cuda::getCurrentCUDAStream(st->device).stream();
     if (at::globalContext().deterministicAlgorithms()) {
         Tensor det = det_scratch(st->n_inst, P * V, f32);
@@ -462,7 +470,7 @@ std::vector<Tensor> views_backward_impl(const std::shared_ptr<ViewsState> &st, c
 
 std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const OptTensor &gC, const OptTensor &gD, const OptTensor &gA,
                                    bool accumulate, const std::vector<OptTensor> &out, bool camera) {
-    return views_backward_impl(st, gC, gD, gA, accumulate, out, c10::nullopt, c10::nullopt, c10::nullopt, 0, camera);
+    return views_backward_impl(st, gC, gD, gA, accumulate, out, c10::nullopt, c10::nullopt, c10::nullopt, 0, camera, c10::nullopt);
 }
 
 }  // namespace
@@ -478,7 +486,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("scales"), py::arg("rots"), py::arg("cov3D"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
     m.def("backward", &backward, "backward through the C ABI", pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"),
           pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"),
-          pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0, pybind11::arg("camera") = false);
+          pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0, pybind11::arg("camera") = false,
+          pybind11::arg("absgrad") = pybind11::none());
     pybind11::class_<ViewsState, std::shared_ptr<ViewsState>>(m, "ViewsState")
         .def_readonly("capacity", &ViewsState::capacity)
         .def_readonly("num_rendered", &ViewsState::n_inst);
@@ -494,7 +503,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("views_mixed_backward", &views_backward_impl, "backward of the batched call with a size per view through the C ABI",
           pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"),
           pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"), pybind11::arg("denom"), pybind11::arg("max_radii2D"),
-          pybind11::arg("stats_views"), pybind11::arg("camera") = false);
+          pybind11::arg("stats_views"), pybind11::arg("camera") = false, pybind11::arg("absgrad") = pybind11::none());
     m.def("set_views_mixed_hint", [](int dev, int64_t P, const std::vector<int32_t> &hw, int64_t cap, bool big) {
         std::lock_guard<std::mutex> lk(g_mu); g_views_mixed_hints[views_mixed_hint_key(dev, P, hw)] = Hint{cap, big}; });
     m.def("get_views_mixed_hint", [](int dev, int64_t P, const std::vector<int32_t> &hw) -> pybind11::object {

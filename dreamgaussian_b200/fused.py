@@ -22,12 +22,15 @@ from . import rasterizer as _r
 
 
 class DensifyStats:
-    """The three per-Gaussian statistics of the reference's densification (float32 [P]; the reference keeps [P,1] / [P])."""
+    """The three per-Gaussian statistics of the reference's densification (float32 [P]; the reference keeps [P,1] / [P]).
+    absgrad=True adds xyz_gradient_accum_abs (float32 [P], else None): AbsGS's statistic, the per-render norm of the summed ABSOLUTE
+    per-pixel terms of dL/dmeans2D (DGR_RASTER_ABS_GRAD, include/dgr_b200.h), which the renders below then update as well."""
 
-    def __init__(self, P: int, device):
+    def __init__(self, P: int, device, absgrad: bool = False):
         self.xyz_gradient_accum = torch.zeros((P,), dtype=torch.float32, device=device)
         self.denom = torch.zeros((P,), dtype=torch.float32, device=device)
         self.max_radii2D = torch.zeros((P,), dtype=torch.float32, device=device)
+        self.xyz_gradient_accum_abs = torch.zeros((P,), dtype=torch.float32, device=device) if absgrad else None
 
     def as_tuple(self):
         return (self.xyz_gradient_accum, self.denom, self.max_radii2D)
@@ -68,7 +71,8 @@ class _RasterizeRaw(torch.autograd.Function):
         cam_needed = any(needs)
         if state.fast is not None:
             stats = ctx.stats.as_tuple() if ctx.stats is not None else (None, None, None)
-            g = _r._FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *stats, camera=cam_needed)
+            absgrad = ctx.stats.xyz_gradient_accum_abs if ctx.stats is not None else None
+            g = _r._FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *stats, camera=cam_needed, absgrad=absgrad)
             cg = _r._camera_input_grads(ctx.cams, needs, g[9:12]) if cam_needed else [None] * len(ctx.cams)
             return (g[0], g[1], g[2], g[8], g[4], g[5], g[6], None, None, None, *cg)
         xyz, dc, _, op, sc, rot, _, rest = state.tensors
@@ -82,8 +86,10 @@ class _RasterizeRaw(torch.autograd.Function):
         d_rest = torch.empty(rest.shape, **f32) if rest is not None else None
         d_op, d_sc, d_rot = torch.empty((P, 1), **f32), torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
         stats = ctx.stats.as_tuple() if ctx.stats is not None else None
+        absgrad = ctx.stats.xyz_gradient_accum_abs if ctx.stats is not None else None
         camera = _r._camera_outputs(0, xyz.device) if cam_needed else None
-        _r.backward_impl(state, gC, gD, gA, d_xyz, d_m2d, d_dc, None, d_op, d_sc, d_rot, None, d_sh_rest=d_rest, densify=stats, camera=camera)
+        _r.backward_impl(state, gC, gD, gA, d_xyz, d_m2d, d_dc, None, d_op, d_sc, d_rot, None, d_sh_rest=d_rest, densify=stats, camera=camera,
+                         absgrad=absgrad)
         cg = _r._camera_input_grads(ctx.cams, needs, camera) if cam_needed else [None] * len(ctx.cams)
         return (d_xyz, d_m2d if ctx.needs_input_grad[1] else None, d_dc, d_rest, d_op, d_sc, d_rot, None, None, None, *cg)
 
@@ -91,7 +97,7 @@ class _RasterizeRaw(torch.autograd.Function):
 class FusedGaussianRasterizer(nn.Module):
     """`GaussianRasterizer` for raw parameters.  forward(xyz, features_dc, features_rest, opacity, scaling, rotation,
     means2D=None, stats=None) -> (color [3,H,W], radii int32 [P], depth [1,H,W], alpha [1,H,W]); `stats` (DensifyStats) is
-    updated during the backward.  antialiasing: as GaussianRasterizer (the 2D Mip filter with opacity compensation).  Camera
+    updated during the backward, its xyz_gradient_accum_abs too when it has one.  antialiasing: as GaussianRasterizer (the 2D Mip filter with opacity compensation).  Camera
     tensors of the settings that require grad receive their gradient, as with GaussianRasterizer."""
 
     def __init__(self, raster_settings: _r.GaussianRasterizationSettings, antialiasing: bool = False):

@@ -170,16 +170,23 @@ def _raster_opts(antialiasing):
     return ctypes.byref(_lib.DgrRasterOptions(_lib.RASTER_ANTIALIAS if antialiasing else 0))
 
 
-def _backward_opts(antialiasing, camera, V, P, dev):
+def _backward_opts(antialiasing, camera, V, P, dev, absgrad=None):
     """The DgrRasterOptions argument of a backward *_ex call.  camera = (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos) float32 outputs
     ([16], [16], [3] or [V,16], [V,16], [V,3]) or None; with them, DGR_RASTER_CAMERA_GRADS and its scratch (the returned pointer
-    keeps the option structs alive, the scratch stays alive until the call returns)."""
-    if camera is None:
+    keeps the option structs alive, the scratch stays alive until the call returns).  absgrad = xyz_gradient_accum_abs float32 [P]
+    or None; with it, DGR_RASTER_ABS_GRAD."""
+    if camera is None and absgrad is None:
         return _raster_opts(antialiasing), None
-    lib = _lib.load()
-    scratch = torch.empty((lib.dgr_camera_grad_scratch_bytes(int(V), int(P)),), dtype=torch.uint8, device=dev)
-    cg = _lib.DgrCameraGrads(*(_ptr(t) for t in camera), _ptr(scratch), scratch.numel())
-    opt = _lib.DgrRasterOptionsCamera((_lib.RASTER_ANTIALIAS if antialiasing else 0) | _lib.RASTER_CAMERA_GRADS, ctypes.pointer(cg))
+    flags = _lib.RASTER_ANTIALIAS if antialiasing else 0
+    cg, scratch = None, None
+    if camera is not None:
+        lib = _lib.load()
+        scratch = torch.empty((lib.dgr_camera_grad_scratch_bytes(int(V), int(P)),), dtype=torch.uint8, device=dev)
+        cg = ctypes.pointer(_lib.DgrCameraGrads(*(_ptr(t) for t in camera), _ptr(scratch), scratch.numel()))
+        flags |= _lib.RASTER_CAMERA_GRADS
+    if absgrad is not None:
+        flags |= _lib.RASTER_ABS_GRAD
+    opt = _lib.DgrRasterOptionsFull(flags, cg, _ptr(absgrad))
     return ctypes.cast(ctypes.pointer(opt), ctypes.POINTER(_lib.DgrRasterOptions)), scratch
 
 
@@ -308,16 +315,17 @@ def _host_sync_objects(dev):
 
 
 def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot,
-                  d_cov, accumulate=False, d_sh_rest=None, densify=None, push=None, camera=None):
+                  d_cov, accumulate=False, d_sh_rest=None, densify=None, push=None, camera=None, absgrad=None):
     """Runs the backward through the C ABI, writing (or accumulating) into the given gradient tensors.
     densify = (xyz_gradient_accum, denom, max_radii2D) float32 [P] tensors (any may be None) updated in the same kernel.
     push = a _lib.DgrPeerPush (multi-GPU: rows of Gaussians another rank owns go straight to that rank, include/dgr_b200.h).
-    camera = (dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3]) float32 tensors, written (never accumulated), or None."""
+    camera = (dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3]) float32 tensors, written (never accumulated), or None.
+    absgrad = xyz_gradient_accum_abs float32 [P], updated with the absolute-gradient statistic (DGR_RASTER_ABS_GRAD), or None."""
     push_addr = ctypes.addressof(push) if push is not None else 0
     if state.fast is not None:
         g = _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate),
                            [d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, d_sh_rest], *(densify or (None, None, None)),
-                           push_addr, camera=camera is not None)
+                           push_addr, camera=camera is not None, absgrad=absgrad)
         if camera is not None:
             for dst, src in zip(camera, g[9:12]):
                 dst.copy_(src)
@@ -333,7 +341,7 @@ def backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2
         args = (ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(state.geom), _ptr(state.binning),
                 ctypes.c_uint64(state.capacity), state.staging, _ptr(state.image), _ptr(state.radii), _ptr(state.alpha),
                 ctypes.byref(gin), ctypes.byref(gout))
-        opts, _scratch = _backward_opts(state.antialiasing, camera, 1, fr.P, dev)
+        opts, _scratch = _backward_opts(state.antialiasing, camera, 1, fr.P, dev, absgrad)
         if torch.are_deterministic_algorithms_enabled():
             det = _det_scratch(lib, state.num_rendered, fr.P, dev)
             _lib.check(lib.dgr_backward_det_ex(*args, *_det_args(det, state.num_rendered), opts, _stream_ptr(dev)))
@@ -631,16 +639,17 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
 
 
 def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot,
-                        accumulate=False, d_sh_rest=None, densify=None, stats_views=0, camera=None):
+                        accumulate=False, d_sh_rest=None, densify=None, stats_views=0, camera=None, absgrad=None):
     """Backward of a batched forward: the per-Gaussian gradients are the sums over the views (written, or added with
     accumulate); d_means2D is per view, [V,P,3].  Mixed-size forwards only: densify = (xyz_gradient_accum, denom, max_radii2D)
-    float32 [P] tensors (any may be None), updated for the views whose bit is set in the stats_views mask.
+    float32 [P] tensors (any may be None), updated for the views whose bit is set in the stats_views mask, and absgrad =
+    xyz_gradient_accum_abs float32 [P] (DGR_RASTER_ABS_GRAD) or None, updated for the same views.
     camera = (dL/dviewmatrix [V,16], dL/dprojmatrix [V,16], dL/dcampos [V,3]) float32 tensors, each view's own, or None."""
     if state.fast is not None:
         outs = [d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest]
         if state.mixed:
             g = _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs,
-                                           *(densify or (None, None, None)), int(stats_views), camera=camera is not None)
+                                           *(densify or (None, None, None)), int(stats_views), camera=camera is not None, absgrad=absgrad)
         else:
             g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, bool(accumulate), outs, camera=camera is not None)
         if camera is not None:
@@ -657,7 +666,7 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
                                      *((_ptr(t) for t in densify) if densify is not None else (None, None, None)), None)
         common = (ctypes.byref(vw.gaussians), _ptr(state.geom), _ptr(state.binning), ctypes.c_uint64(state.capacity), state.staging,
                   _ptr(state.image), _ptr(state.radii), ctypes.byref(gin), ctypes.byref(gout))
-        opts, _scratch = _backward_opts(state.antialiasing, camera, vw.V, vw.P, dev)
+        opts, _scratch = _backward_opts(state.antialiasing, camera, vw.V, vw.P, dev, absgrad)
         if torch.are_deterministic_algorithms_enabled():
             det = _det_scratch(lib, state.num_rendered, vw.P * vw.V, dev)
             if state.mixed:
@@ -677,12 +686,14 @@ def views_backward_impl(state, grad_color, grad_depth, grad_alpha, d_means3D, d_
 def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, stats_views=0, camera=False):
     """-> (means3D, means2D [V,P,3], shs | features_dc, features_rest, opacities, scales, rotations) gradients, and with camera=True
     also (dL/dviewmatrix [V,16], dL/dprojmatrix [V,16], dL/dcampos [V,3]) as an 8th element.
-    stats (DensifyStats) / stats_views (bit mask): the densification statistics of a mixed-size forward."""
+    stats (DensifyStats) / stats_views (bit mask): the densification statistics of a mixed-size forward (with the absolute-gradient
+    one when stats carries it)."""
     densify = stats.as_tuple() if stats is not None else None
+    absgrad = stats.xyz_gradient_accum_abs if stats is not None else None
     if state.fast is not None:
         if state.mixed:
             g = _FAST.views_mixed_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], *(densify or (None, None, None)),
-                                           int(stats_views) if densify is not None else 0, camera=bool(camera))
+                                           int(stats_views) if densify is not None else 0, camera=bool(camera), absgrad=absgrad)
         else:
             g = _FAST.views_backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], camera=bool(camera))   # undefined -> None
         out = (g[0], g[1], g[2], g[6], g[3], g[4], g[5])
@@ -700,7 +711,7 @@ def _views_grads(state, grad_color, grad_depth, grad_alpha, raw, stats=None, sta
     d_scales, d_rot = torch.empty((P, 3), **f32), torch.empty((P, 4), **f32)
     cam = _camera_outputs(V, means3D.device) if camera else None
     views_backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_opac, d_scales, d_rot, d_sh_rest=d_rest, densify=densify,
-                        stats_views=stats_views if densify is not None else 0, camera=cam)
+                        stats_views=stats_views if densify is not None else 0, camera=cam, absgrad=absgrad)
     out = (d_means3D, d_means2D, d_sh, d_rest, d_opac, d_scales, d_rot)
     return out + (cam,) if camera else out
 

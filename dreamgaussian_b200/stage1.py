@@ -79,6 +79,7 @@ class GaussianModelB200:
         self.lr = {}
         self.steps = {k: 0 for k in GROUPS}          # torch.optim.Adam keeps state['step'] per tensor
         self.stats: Optional[DensifyStats] = None
+        self.absgrad = False                       # keep AbsGS's statistic too (DensifyStats.xyz_gradient_accum_abs)
         self.percent_dense = 0.01
         self.spatial_lr_scale = 1.0
         self.betas, self.eps = (0.9, 0.999), 1e-15
@@ -123,7 +124,7 @@ class GaussianModelB200:
                                                max_steps=cfg.position_lr_max_steps)
 
     def _reset_stats(self):
-        self.stats = DensifyStats(self.num_points, self.p["xyz"].device)
+        self.stats = DensifyStats(self.num_points, self.p["xyz"].device, absgrad=self.absgrad)
 
     def update_learning_rate(self, iteration):
         self.lr["xyz"] = self.xyz_scheduler(iteration)
@@ -176,6 +177,8 @@ class GaussianModelB200:
             self.exp_avg_sq = {k: v[mask].contiguous() for k, v in self.exp_avg_sq.items()}
             st = self.stats
             st.xyz_gradient_accum, st.denom, st.max_radii2D = st.xyz_gradient_accum[mask], st.denom[mask], st.max_radii2D[mask]
+            if st.xyz_gradient_accum_abs is not None:
+                st.xyz_gradient_accum_abs = st.xyz_gradient_accum_abs[mask]
 
     def _append(self, new):
         """densification_postfix + cat_tensors_to_optimizer (:515-552): new points get zero Adam moments, stats reset."""
@@ -221,10 +224,11 @@ class GaussianModelB200:
             m = m | (self.stats.max_radii2D > max_screen_size) | (torch.exp(self.p["scaling"].detach()).max(dim=1).values > 0.1 * extent)
         return m
 
-    def _densify_fused(self, max_grad, min_opacity, extent, max_screen_size, noise=None):
+    def _densify_fused(self, max_grad, min_opacity, extent, max_screen_size, noise=None, max_abs_grad=None):
         """densify_and_prune as two launches of compaction kernels (csrc/dgr_densify.cuh: classify + block scan, then ONE pass
         that writes the six parameter tensors and both Adam moments in the reference's final order) with one host read-back
-        of the new point count between them — instead of ~30 boolean-mask indexing / torch.cat calls."""
+        of the new point count between them — instead of ~30 boolean-mask indexing / torch.cat calls.  max_abs_grad: split by
+        the absolute-gradient statistic (dgr_densify_plan_ex)."""
         lib = _lib.load()
         P, dev = self.num_points, self.p["xyz"].device
         with torch.no_grad(), torch.cuda.device(dev):
@@ -233,9 +237,16 @@ class GaussianModelB200:
             if getattr(self, "_counts_host", None) is None:
                 self._counts_host = torch.zeros((4,), dtype=torch.int32).pin_memory()
             acc, den = self.stats.xyz_gradient_accum.contiguous(), self.stats.denom.contiguous()
-            _lib.check(lib.dgr_densify_plan(P, acc.data_ptr(), den.data_ptr(), self.p["opacity"].data_ptr(), self.p["scaling"].data_ptr(),
-                                            float(max_grad), float(self.percent_dense * extent), float(min_opacity), float(0.1 * extent),
-                                            1 if max_screen_size else 0, scratch.data_ptr(), self._counts_host.data_ptr(), st))
+            if max_abs_grad is None:
+                _lib.check(lib.dgr_densify_plan(P, acc.data_ptr(), den.data_ptr(), self.p["opacity"].data_ptr(), self.p["scaling"].data_ptr(),
+                                                float(max_grad), float(self.percent_dense * extent), float(min_opacity), float(0.1 * extent),
+                                                1 if max_screen_size else 0, scratch.data_ptr(), self._counts_host.data_ptr(), st))
+            else:
+                acc_abs = self.stats.xyz_gradient_accum_abs.contiguous()
+                _lib.check(lib.dgr_densify_plan_ex(P, acc.data_ptr(), acc_abs.data_ptr(), den.data_ptr(), self.p["opacity"].data_ptr(),
+                                                   self.p["scaling"].data_ptr(), float(max_grad), float(max_abs_grad),
+                                                   float(self.percent_dense * extent), float(min_opacity), float(0.1 * extent),
+                                                   1 if max_screen_size else 0, scratch.data_ptr(), self._counts_host.data_ptr(), st))
             torch.cuda.current_stream(dev).synchronize()
             n_keep, n_clone, n_sel, n_child = (int(x) for x in self._counts_host)
             n_out = n_keep + n_clone + 2 * n_child
@@ -259,14 +270,24 @@ class GaussianModelB200:
             self.exp_avg, self.exp_avg_sq = new_m, new_v
         self._reset_stats()
 
-    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, noise=None):
+    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, noise=None, max_abs_grad=None):
+        """max_abs_grad (needs stats with xyz_gradient_accum_abs): AbsGS's rule (Ye et al., 2024) — clone by the default statistic,
+        split by the absolute one (xyz_gradient_accum_abs / denom >= max_abs_grad)."""
+        if max_abs_grad is not None and self.stats.xyz_gradient_accum_abs is None:
+            raise ValueError("densify_and_prune: max_abs_grad needs the absolute-gradient statistic (GaussianModelB200.absgrad = True)")
         if getattr(self, "fused_densify", False) and self.p["xyz"].is_cuda and self.num_points > 0:
-            return self._densify_fused(max_grad, min_opacity, extent, max_screen_size, noise=noise)
+            return self._densify_fused(max_grad, min_opacity, extent, max_screen_size, noise=noise, max_abs_grad=max_abs_grad)
         with torch.no_grad():
             grads = self.stats.xyz_gradient_accum / self.stats.denom
             grads[grads.isnan()] = 0.0
+            if max_abs_grad is not None:
+                grads_abs = self.stats.xyz_gradient_accum_abs / self.stats.denom
+                grads_abs[grads_abs.isnan()] = 0.0
         self.densify_and_clone(grads, max_grad, extent)
-        self.densify_and_split(grads, max_grad, extent, noise=noise)
+        if max_abs_grad is None:
+            self.densify_and_split(grads, max_grad, extent, noise=noise)
+        else:
+            self.densify_and_split(grads_abs, max_abs_grad, extent, noise=noise)
         self.prune_points(self._prune_mask(min_opacity, extent, max_screen_size))
 
     def prune(self, min_opacity, extent, max_screen_size):
@@ -304,6 +325,9 @@ class Stage1Config(NamedTuple):
     densify_grad_threshold: float = 0.01
     seed: int = 0
     antialiasing: bool = False          # every render with the 2D Mip filter and opacity compensation (GaussianRasterizer's switch)
+    # AbsGS densification: split by the absolute-gradient statistic at this threshold (clone as before); None = the default loop.
+    # Needs fused=True: the statistic exists only inside the backward render.
+    densify_abs_grad_threshold: Optional[float] = None
 
 
 class GuidanceStub:
@@ -342,6 +366,9 @@ class Stage1Trainer:
         from . import scene
         if batched and not fused:
             raise ValueError("Stage1Trainer: batched=True needs fused=True (the batched call takes the raw parameters)")
+        if cfg.densify_abs_grad_threshold is not None and not fused:
+            raise ValueError("Stage1Trainer: densify_abs_grad_threshold needs fused=True (the reference formulation takes its statistics "
+                             "from means2D.grad, which has no per-pixel absolute values)")
         self.cfg, self.device, self.fused, self.batched = cfg, torch.device(device), fused, batched
         self.rng = np.random.default_rng(cfg.seed)
         self.scene = scene
@@ -350,6 +377,7 @@ class Stage1Trainer:
         self.gaussians = GaussianModelB200(cfg.sh_degree)
         self.gaussians.fused_adam = fused
         self.gaussians.fused_densify = fused
+        self.gaussians.absgrad = cfg.densify_abs_grad_threshold is not None
         # the split children's noise comes from the trainer's own generator: torch's default one is seeded differently in every
         # process, so two runs from one seed would split differently at the first densification
         self.gaussians.noise_gen = torch.Generator(device=self.device).manual_seed(cfg.seed)
@@ -406,7 +434,8 @@ class Stage1Trainer:
                     st.xyz_gradient_accum[vis] += torch.norm(self._last["viewspace_points"].grad[vis, :2], dim=-1)
                     st.denom[vis] += 1
             if self.step % cfg.densification_interval == 0:
-                g.densify_and_prune(cfg.densify_grad_threshold, min_opacity=0.01, extent=4, max_screen_size=1)
+                g.densify_and_prune(cfg.densify_grad_threshold, min_opacity=0.01, extent=4, max_screen_size=1,
+                                    max_abs_grad=cfg.densify_abs_grad_threshold)
             if self.step % cfg.opacity_reset_interval == 0:          # main.py:285-286 (700 > 500 iterations in image.yaml)
                 g.reset_opacity()
         self._last = None

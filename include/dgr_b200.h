@@ -333,9 +333,31 @@ typedef struct DgrCameraGrads {
     uint64_t scratch_bytes;
 } DgrCameraGrads;
 size_t dgr_camera_grad_scratch_bytes(int32_t V, int32_t P);
+/* == Absolute-gradient densification statistic (DGR_RASTER_ABS_GRAD, backward *_ex calls only; AbsGS, Ye et al., 2024) ==
+ * xyz_gradient_accum adds |dL/dmeans2D[:2]| per render: the norm of a SUM over the pixels a Gaussian covers, which cancels where
+ * those pixels pull its centre in opposite directions.  With the bit, the backward also adds, for every Gaussian with radius > 0
+ * in the render (dgr_views_mixed_backward*: in each view whose bit is set in stats_views, in view order),
+ *   xyz_gradient_accum_abs[g] += sqrt(a_x^2 + a_y^2),   a_x = sum_p |u_p (A dx + B dy)| W/2,   a_y = sum_p |u_p (B dx + C dy)| H/2
+ * over the pixels p where the backward render evaluates g (its gradient's pixels and skip rules), u_p = o G_p dL/dalpha_p (o_eff
+ * with DGR_RASTER_ANTIALIAS; min(0.99, .) straight-through), (dx, dy) = mean - pixel, (A, B, C) the conic: NDC units like
+ * dL/dmeans2D, and >= the xyz_gradient_accum term of the same render (triangle inequality; equal for a one-pixel Gaussian).
+ * xyz_gradient_accum_abs: device float32 [P], read only with the bit.  Gradients and the three other statistics are those of the
+ * call without the bit, up to the order of float additions (the backward render runs its ABS variant of the default sub-tile
+ * shape whatever dgr_set_tuning says); the *_det calls keep their bit-reproducibility for the new statistic too.  Accepted by
+ * dgr_backward_ex, dgr_backward_det_ex, dgr_views_mixed_backward_ex and dgr_views_mixed_backward_det_ex, combined with
+ * DGR_RASTER_ANTIALIAS and DGR_RASTER_CAMERA_GRADS as wanted.  Refused before any device work, each with its own dgr_last_error
+ * text: the bit on a forward call, the bit with xyz_gradient_accum_abs == NULL, the bit on dgr_views_backward_ex /
+ * dgr_views_backward_det_ex (the same-size batch has no statistics), and the bit on a mixed call with stats_views == 0.
+ * Bits 2u and 8u stay unknown (refused), so a DgrRasterOptions that ends after `flags` or after `camera` is never read past its
+ * end; a caller that sets this bit passes the whole struct.
+ * Cost: the ABS render variant (about 4 more floating-point instructions per record and pixel in step 2) and one kernel of one
+ * thread per Gaussian after the per-Gaussian backward (absgrad_stats); DESIGN.md §4 has the times.  Densify with
+ * dgr_densify_plan_ex. */
+#define DGR_RASTER_ABS_GRAD 16u
 typedef struct DgrRasterOptions {
     uint32_t flags;          /* DGR_RASTER_* bits */
     const DgrCameraGrads *camera;   /* read only when flags has DGR_RASTER_CAMERA_GRADS */
+    float *xyz_gradient_accum_abs;  /* [P], read only when flags has DGR_RASTER_ABS_GRAD */
 } DgrRasterOptions;
 int dgr_forward_preprocess_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii,
                               const DgrRasterOptions *opt, void *stream);
@@ -448,6 +470,13 @@ int dgr_densify_plan(int32_t P, const float *xyz_gradient_accum, const float *de
                      float grad_threshold, float dense_extent, float min_opacity, float max_world, int32_t use_world,
                      void *scratch, uint32_t *counts_host, void *stream);
 int dgr_densify_apply(int32_t P, const DgrDensifyTensors *t, const float *noise, const void *scratch, void *stream);
+/* dgr_densify_plan with AbsGS's rule (DGR_RASTER_ABS_GRAD): clone as dgr_densify_plan (grad >= grad_threshold and small), split
+ * when xyz_gradient_accum_abs / denom (NaN -> 0) >= abs_grad_threshold and max(exp(scaling)) > dense_extent; the prune rules, the
+ * counts and dgr_densify_apply are unchanged.  xyz_gradient_accum_abs must not be NULL when P > 0. */
+int dgr_densify_plan_ex(int32_t P, const float *xyz_gradient_accum, const float *xyz_gradient_accum_abs, const float *denom,
+                        const float *opacity_raw, const float *scaling_raw, float grad_threshold, float abs_grad_threshold,
+                        float dense_extent, float min_opacity, float max_world, int32_t use_world, void *scratch,
+                        uint32_t *counts_host, void *stream);
 
 /* GaussianRasterizer.markVisible: present[i] = 1 if Gaussian i passes the near-plane test. */
 int dgr_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
