@@ -90,9 +90,22 @@ class DgrRasterOptionsFull(ctypes.Structure):
     _fields_ = [("flags", ctypes.c_uint32), ("camera", ctypes.POINTER(DgrCameraGrads)), ("xyz_gradient_accum_abs", c_f32p)]
 
 
+class DgrContrib(ctypes.Structure):
+    """Outputs of DGR_RASTER_CONTRIB (include/dgr_b200.h): weight_sum / weight_max float32 [records] and their scratch."""
+    _fields_ = [("weight_sum", c_f32p), ("weight_max", c_f32p), ("scratch", ctypes.c_void_p), ("scratch_bytes", ctypes.c_uint64)]
+
+
+class DgrRasterOptionsContrib(ctypes.Structure):
+    """DgrRasterOptions with all three trailing members; the stage-2 render *_ex calls read `contrib` only with
+    DGR_RASTER_CONTRIB.  Pass it cast to POINTER(DgrRasterOptions)."""
+    _fields_ = [("flags", ctypes.c_uint32), ("camera", ctypes.POINTER(DgrCameraGrads)), ("xyz_gradient_accum_abs", c_f32p),
+                ("contrib", ctypes.POINTER(DgrContrib))]
+
+
 RASTER_ANTIALIAS = 1                 # DGR_RASTER_ANTIALIAS
 RASTER_CAMERA_GRADS = 4              # DGR_RASTER_CAMERA_GRADS (backward *_ex calls only)
 RASTER_ABS_GRAD = 16                 # DGR_RASTER_ABS_GRAD (backward *_ex calls only)
+RASTER_CONTRIB = 32                  # DGR_RASTER_CONTRIB (stage-2 render *_ex calls only)
 
 VIEWS_MAX = 64                       # DGR_VIEWS_MAX
 VIEWS_MAX_RECORDS = 2 ** 31 - 1      # DGR_VIEWS_MAX_RECORDS: V x P
@@ -117,6 +130,7 @@ EXPORTS = (
     "dgr_backward_ex", "dgr_views_backward_ex", "dgr_views_mixed_backward_ex",
     "dgr_backward_det_ex", "dgr_views_backward_det_ex", "dgr_views_mixed_backward_det_ex",
     "dgr_camera_grad_scratch_bytes", "dgr_densify_plan_ex",
+    "dgr_contrib_scratch_bytes", "dgr_forward_render_ex", "dgr_views_forward_render_ex", "dgr_views_mixed_forward_render_ex",
 )
 
 _lib = None
@@ -240,12 +254,14 @@ def load():
     # the *_ex calls: the counterpart's arguments + const DgrRasterOptions * (NULL = flags 0) before the stream
     for name in ("dgr_forward_preprocess", "dgr_views_forward_preprocess", "dgr_views_mixed_forward_preprocess", "dgr_backward",
                  "dgr_views_backward", "dgr_views_mixed_backward", "dgr_backward_det", "dgr_views_backward_det",
-                 "dgr_views_mixed_backward_det"):
+                 "dgr_views_mixed_backward_det", "dgr_forward_render", "dgr_views_forward_render", "dgr_views_mixed_forward_render"):
         ex = getattr(lib, name + "_ex")
         ex.restype = ctypes.c_int
         ex.argtypes = list(getattr(lib, name).argtypes[:-1]) + [ctypes.POINTER(DgrRasterOptions), vp]
     lib.dgr_camera_grad_scratch_bytes.restype = ctypes.c_size_t
     lib.dgr_camera_grad_scratch_bytes.argtypes = [i32, i32]
+    lib.dgr_contrib_scratch_bytes.restype = ctypes.c_size_t
+    lib.dgr_contrib_scratch_bytes.argtypes = [ctypes.c_int64]
     if lib.dgr_abi_version() != ABI_VERSION:
         raise RuntimeError("libdgr_b200.so ABI version mismatch")
     _lib = lib

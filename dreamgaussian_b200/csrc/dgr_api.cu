@@ -174,8 +174,44 @@ int raster_flags(const DgrRasterOptions *opt, uint32_t *flags) {
     *flags = opt ? opt->flags : 0u;
     if (*flags & DGR_RASTER_CAMERA_GRADS) return fail(-1, "DgrRasterOptions: DGR_RASTER_CAMERA_GRADS is backward-only (a forward call refuses it)");
     if (*flags & DGR_RASTER_ABS_GRAD) return fail(-1, "DgrRasterOptions: DGR_RASTER_ABS_GRAD is backward-only (a forward call refuses it)");
+    if (*flags & DGR_RASTER_CONTRIB) return fail(-1, "DgrRasterOptions: DGR_RASTER_CONTRIB belongs to the stage-2 render calls (a preprocess call refuses it)");
     if (*flags & ~DGR_RASTER_ANTIALIAS) return fail(-1, "DgrRasterOptions: unknown flag bits");
     return 0;
+}
+// The stage-2 render calls' options: DGR_RASTER_CONTRIB only (*cb: the statistics' outputs, NULL without the bit), checked
+// against `records` (P, or V P).
+int raster_flags_render(const DgrRasterOptions *opt, int64_t records, const DgrContrib **cb) {
+    const uint32_t flags = opt ? opt->flags : 0u;
+    *cb = nullptr;
+    if (flags & ~DGR_RASTER_CONTRIB) return fail(-1, "DgrRasterOptions: a stage-2 render call accepts DGR_RASTER_CONTRIB only");
+    if (!(flags & DGR_RASTER_CONTRIB)) return 0;
+    const DgrContrib *c = opt->contrib;
+    if (!c) return fail(-1, "DgrRasterOptions: DGR_RASTER_CONTRIB with contrib == NULL");
+    if (!c->weight_sum || !c->weight_max) return fail(-1, "contribution statistics: weight_sum / weight_max is NULL");
+    if (!c->scratch) return fail(-1, "contribution statistics: scratch is NULL");
+    if (c->scratch_bytes < dgr_contrib_scratch_bytes(records))
+        return fail(-1, "contribution statistics: scratch is smaller than dgr_contrib_scratch_bytes(records)");
+    *cb = c;
+    return 0;
+}
+// DGR_RASTER_CONTRIB, before the render of every stage-2 run: outputs and scratch zeroed, so the run's values are its own
+int contrib_clear(const DgrContrib *cb, int64_t records, cudaStream_t st) {
+    if (!cb || records == 0) return 0;
+    DGR_CUDA(cudaMemsetAsync(cb->weight_max, 0, (size_t)records * 4, st));
+    DGR_CUDA(cudaMemsetAsync(cb->scratch, 0, (size_t)records * 8, st));
+    return 0;
+}
+// ... and after it: the fixed-point sums -> weight_sum
+int contrib_finalize(const DgrContrib *cb, int64_t records, int debug, cudaStream_t st) {
+    if (!cb || records == 0) return 0;
+    DGR_KERNEL("contrib_finalize", st, debug,
+               launch_k(contrib_finalize_kernel, dim3((unsigned)((records + kContribFinalizeThreads - 1) / kContribFinalizeThreads)),
+                        dim3(kContribFinalizeThreads), 0, st, false, (long long)records,
+                        (const unsigned long long *)cb->scratch, cb->weight_sum));
+    return 0;
+}
+ContribOut contrib_out(const DgrContrib *cb) {
+    return ContribOut{reinterpret_cast<unsigned long long *>(cb->scratch), reinterpret_cast<unsigned *>(cb->weight_max)};
 }
 // The backward calls' options: the recorded / compared flags (DGR_RASTER_ANTIALIAS), with DGR_RASTER_CAMERA_GRADS the camera
 // outputs (*cam; NULL without the bit) and with DGR_RASTER_ABS_GRAD the absolute-gradient statistic (*abs_accum; NULL without it).
@@ -183,6 +219,7 @@ int raster_flags_bwd(const DgrRasterOptions *opt, uint32_t *flags, const DgrCame
     *flags = opt ? opt->flags : 0u;
     *cam = nullptr;
     *abs_accum = nullptr;
+    if (*flags & DGR_RASTER_CONTRIB) return fail(-1, "DgrRasterOptions: DGR_RASTER_CONTRIB belongs to the stage-2 render calls (a backward call refuses it)");
     if (*flags & ~(DGR_RASTER_ANTIALIAS | DGR_RASTER_CAMERA_GRADS | DGR_RASTER_ABS_GRAD)) return fail(-1, "DgrRasterOptions: unknown flag bits");
     if (*flags & DGR_RASTER_CAMERA_GRADS) {
         if (!opt->camera) return fail(-1, "DgrRasterOptions: DGR_RASTER_CAMERA_GRADS with camera == NULL");
@@ -636,12 +673,13 @@ int dgr_forward_preprocess_ex(const DgrSettings *s, const DgrGaussians *g, void 
     return forward_preprocess(s, g, geom_v, image_v, radii, flags, stream);
 }
 
-int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
-                       void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
-                       void *count_ready_event, void *stream) {
-    NvtxRange nvtx_("dgr_forward_render");
+static int forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                          void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                          void *count_ready_event, const DgrRasterOptions *opt, void *stream) {
     if (int e = check_settings(s)) return e;
     if (!g || !geom_v || !image_v || !out) return fail(-1, "NULL argument");
+    const DgrContrib *cb = nullptr;
+    if (int e = raster_flags_render(opt, g->P, &cb)) return e;
     if (!out->color || !out->depth || !out->alpha) return fail(-1, "output images must not be NULL");
     if (capacity > 0 && !binning_v) return fail(-1, "binning scratch is NULL");
     if (capacity >= 0xffffffffull) return fail(-3, "capacity above 2^32-1 tile instances not supported");
@@ -671,6 +709,7 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v
     if (!dv) return -1;
     if (flags & DGR_FLAG_RERUN)
         if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
+    if (int e = contrib_clear(cb, g->P, st)) return e;
     {
         // instance emission; its extra block publishes ranges / order / counts (capacity 0: only that block has work to do)
         const size_t smem = (size_t)tiles * 4;
@@ -701,13 +740,44 @@ int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v
                             s->bg, out->color, out->depth, out->alpha, n_contrib, final_T));                     \
     } while (0)
 #define DGR_RENDER_FWD(PPL_, U_) do { if (lazy) DGR_RENDER_FWD_L(PPL_, U_, true); else DGR_RENDER_FWD_L(PPL_, U_, false); } while (0)
-    if (ppl == 4) DGR_RENDER_FWD(4, 1);
+    // DGR_RASTER_CONTRIB: the default shape's statistics variant, whatever the knobs
+#define DGR_RENDER_FWD_C(L_)                                                                                    \
+    do {                                                                                                        \
+        const int items_ = tiles * SubTile<1>::kPerTile;                                                        \
+        int grid_ = min(persistent_grid(dv, render_fwd_contrib_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
+        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                               \
+        DGR_KERNEL("render_fwd_contrib", st, s->debug,                                                          \
+                   launch_k(render_fwd_contrib_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, H, W, IL.gx, \
+                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),         \
+                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
+                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids,                                      \
+                            s->bg, out->color, out->depth, out->alpha, n_contrib, final_T, contrib_out(cb)));    \
+    } while (0)
+    if (cb) { if (lazy) DGR_RENDER_FWD_C(true); else DGR_RENDER_FWD_C(false); }
+    else if (ppl == 4) DGR_RENDER_FWD(4, 1);
     else if (ppl == 2) DGR_RENDER_FWD(2, 2);
     else { if (uf == 4) DGR_RENDER_FWD(1, 4); else DGR_RENDER_FWD(1, 1); }      // default <1,1>: 58 registers, 8 CTAs per SM, no spill
 #undef DGR_RENDER_FWD_L
 #undef DGR_RENDER_FWD
-    return 0;
+#undef DGR_RENDER_FWD_C
+    return contrib_finalize(cb, g->P, s->debug, st);
 }
+
+int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                       void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                       void *count_ready_event, void *stream) {
+    NvtxRange nvtx_("dgr_forward_render");
+    return forward_render(s, g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket, count_ready_event, nullptr, stream);
+}
+
+int dgr_forward_render_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                          void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                          void *count_ready_event, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_forward_render_ex");
+    return forward_render(s, g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket, count_ready_event, opt, stream);
+}
+
+size_t dgr_contrib_scratch_bytes(int64_t records) { return records > 0 ? align_up((size_t)records * 8, 256) : 0; }
 
 static int check_push(const DgrPeerPush *p, int64_t P) {
     if (!p) return 0;
@@ -1049,8 +1119,11 @@ int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians 
 
 int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
                  void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket, void *count_ready_event,
-                 void *stream) {
+                 const DgrRasterOptions *opt, void *stream) {
     if (!geom_v || !image_v || !out) return fail(-1, "NULL argument");
+    const int64_t records = (int64_t)g->P * s->V;
+    const DgrContrib *cb = nullptr;
+    if (int e = raster_flags_render(opt, records, &cb)) return e;
     if (!out->color || !out->depth || !out->alpha) return fail(-1, "output images must not be NULL");
     if (capacity > 0 && !binning_v) return fail(-1, "binning scratch is NULL");
     if (capacity >= 0xffffffffull) return fail(-3, "capacity above 2^32-1 tile instances not supported");
@@ -1075,6 +1148,7 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
     if (!dv) return -1;
     if (flags & DGR_FLAG_RERUN)
         if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
+    if (int e = contrib_clear(cb, records, st)) return e;
     {
         const int nb = (g->P > 0 && capacity > 0) ? GL.nblocks : 0;
         DGR_KERNEL("emit_views", st, s->debug,
@@ -1100,9 +1174,24 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
                             &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids, s->bg, out->color, out->depth, out->alpha, \
                             reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT))); \
     } while (0)
-    if (lazy) DGR_VIEWS_FWD(true); else DGR_VIEWS_FWD(false);
+#define DGR_VIEWS_FWD_C(L_)                                                                                                 \
+    do {                                                                                                                   \
+        const int items_ = tiles * SubTile<1>::kPerTile;                                                                   \
+        int grid_ = min(persistent_grid(dv, render_views_fwd_contrib_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
+        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                                          \
+        DGR_KERNEL("render_views_fwd_contrib", st, s->debug,                                                               \
+                   launch_k(render_views_fwd_contrib_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, b.vt, \
+                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),          \
+                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
+                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids, s->bg, out->color, out->depth, out->alpha, \
+                            reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT), \
+                            contrib_out(cb)));                                                                               \
+    } while (0)
+    if (cb) { if (lazy) DGR_VIEWS_FWD_C(true); else DGR_VIEWS_FWD_C(false); }
+    else if (lazy) DGR_VIEWS_FWD(true); else DGR_VIEWS_FWD(false);
 #undef DGR_VIEWS_FWD
-    return 0;
+#undef DGR_VIEWS_FWD_C
+    return contrib_finalize(cb, records, s->debug, st);
 }
 
 int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -1203,7 +1292,17 @@ int dgr_views_forward_render(const DgrViews *s, const DgrGaussians *g, void *geo
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     return views_render(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket,
-                        count_ready_event, stream);
+                        count_ready_event, nullptr, stream);
+}
+
+int dgr_views_forward_render_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
+                                void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                                void *count_ready_event, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_forward_render_ex");
+    if (int e = check_views(s)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_render(s, views_batch_uniform(s), g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket,
+                        count_ready_event, opt, stream);
 }
 
 static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1300,7 +1399,17 @@ int dgr_views_mixed_forward_render(const DgrViews *s, const int32_t *image_hw, c
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     return views_render(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket,
-                        count_ready_event, stream);
+                        count_ready_event, nullptr, stream);
+}
+
+int dgr_views_mixed_forward_render_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, void *binning_v,
+                                      uint64_t capacity, void *image_v, const DgrImages *out, int32_t flags, uint64_t *counts_host,
+                                      uint64_t ticket, void *count_ready_event, const DgrRasterOptions *opt, void *stream) {
+    NvtxRange nvtx_("dgr_views_mixed_forward_render_ex");
+    if (int e = check_views_mixed(s, image_hw)) return e;
+    if (int e = check_views_gaussians(s, g)) return e;
+    return views_render(s, views_batch(s->V, image_hw, 2), g, geom_v, binning_v, capacity, image_v, out, flags, counts_host, ticket,
+                        count_ready_event, opt, stream);
 }
 
 static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,

@@ -170,7 +170,20 @@ struct CostOrder {                       // image scratch pieces (all may be NUL
 // VIEWS: a batch of V views (dgr_views_forward_render, dgr_views_mixed_forward_render), each with its own image size (ViewTable
 // vt; H, W, gx unused).  A work item's global tile gives its view (view_of_tile: once per item) and local tile; every view has its
 // own background (bg [V,3]) and its own blocks of the flat images at pix_off[v]; the records are those of the batch.
-template <int PPL, int U, bool LAZY, bool VIEWS>
+//
+// CONTRIB (DGR_RASTER_CONTRIB, render_*_fwd_contrib_kernel only): for every record the warp composites, the weights w = alpha T of
+// its composited pixels are reduced over the warp right after the record (a shuffle butterfly for the sum, redux.sync on the float
+// bits for the max: both a fixed order, so the item's partial is a pure function of the inputs), parked in the lane of the
+// record's chunk slot, and after the chunk that lane adds the partial to the record's 64-bit fixed-point sum (integer atomics:
+// the total does not depend on the order the items arrive in) and raises its max (atomicMax on the bits of a non-negative float).
+struct ContribOut {
+    unsigned long long *sum_fx;          // [records] sum of w, fixed point (kContribScale)
+    unsigned *max_bits;                  // [records] bits of max w (float, >= 0)
+};
+constexpr float kContribScale = 274877906944.f;                  // 2^38
+constexpr float kContribUnscale = 1.f / 274877906944.f;
+
+template <int PPL, int U, bool LAZY, bool VIEWS, bool CONTRIB = false>
 __device__ __forceinline__ void
 render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
                   const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
@@ -178,7 +191,7 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                   const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
                   const float *__restrict__ bg, float *__restrict__ out_color,
                   float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
-                  float *__restrict__ final_T, const ViewTable *vt) {
+                  float *__restrict__ final_T, const ViewTable *vt, ContribOut cw = ContribOut{nullptr, nullptr}) {
     using ST = SubTile<PPL>;
     __shared__ WarpRing rings[kRenderWarps];
     const int lane = threadIdx.x & 31;
@@ -268,6 +281,9 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
             if (lane < cnt) hit = record_hits_subtile(rg.rec[s][lane], wx0, wx1, wy0, wy1);
             unsigned mask = __ballot_sync(0xffffffffu, hit);
             cost += 2u + 4u * (unsigned)__popc(mask);
+            unsigned cid = 0, cmax = 0;                          // CONTRIB: this lane's record of the chunk, its partial
+            float csum = 0.f;
+            if constexpr (CONTRIB) { if (hit) cid = __ldg(ids + c * kChunk + lane); }
             while (mask) {
                 int js[U];
                 int nh = 0;
@@ -297,6 +313,7 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
 #pragma unroll
                 for (int u = 0; u < U; u++) {
                     if (u < nh) {
+                        float lsum = 0.f, lmax = 0.f;           // CONTRIB: this lane's pixels
 #pragma unroll
                         for (int p = 0; p < PPL; p++) {
                             const float a = av[u][p];
@@ -309,9 +326,25 @@ render_fwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                                 D[p] = __fmaf_rn(dep[u], w, D[p]);
                                 T[p] = test_T;
                                 last[p] = (unsigned)(c * kChunk + js[u] + 1);
+                                if constexpr (CONTRIB) { lsum = __fadd_rn(lsum, w); lmax = fmaxf(lmax, w); }
+                            }
+                        }
+                        if constexpr (CONTRIB) {
+                            // w > 0 wherever the record is composited (alpha >= 1/255, T >= 1e-4): max 0 = not composited here
+                            if (__any_sync(0xffffffffu, lmax > 0.f)) {
+#pragma unroll
+                                for (int o = 16; o > 0; o >>= 1) lsum = __fadd_rn(lsum, __shfl_xor_sync(0xffffffffu, lsum, o));
+                                const unsigned m = __reduce_max_sync(0xffffffffu, __float_as_uint(lmax));
+                                if (lane == js[u]) { csum = lsum; cmax = m; }
                             }
                         }
                     }
+                }
+            }
+            if constexpr (CONTRIB) {
+                if (cmax) {
+                    atomicAdd(cw.sum_fx + cid, __float2ull_rn(__fmul_rn(csum, kContribScale)));
+                    atomicMax(cw.max_bits + cid, cmax);
                 }
             }
             all_done = true;
@@ -412,6 +445,40 @@ render_views_fwd_kernel(const __grid_constant__ ViewTable vt, const unsigned *__
                   float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
                   float *__restrict__ final_T) {
     render_fwd_body<1, 1, LAZY, true>(0, 0, 0, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, &vt);
+}
+
+// DGR_RASTER_CONTRIB: the default shape <1,1> with the blending-weight statistics (single view and batched).  Separate kernels,
+// so every instantiation above stays as it was.
+template <bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads, 8)
+render_fwd_contrib_kernel(int H, int W, int gx, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+                  const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
+                  int two_ended, int sms, CostOrder co, unsigned *__restrict__ lazy_note,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
+                  const float *__restrict__ bg, float *__restrict__ out_color,
+                  float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
+                  float *__restrict__ final_T, ContribOut cw) {
+    render_fwd_body<1, 1, LAZY, false, true>(H, W, gx, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, nullptr, cw);
+}
+
+template <bool LAZY>
+__global__ void __launch_bounds__(kRenderThreads, 8)
+render_views_fwd_contrib_kernel(const __grid_constant__ ViewTable vt, const unsigned *__restrict__ tile_order, const uint2 *__restrict__ order_ranges,
+                  const unsigned *__restrict__ n_tiles_nonempty, unsigned n_items, unsigned long long *__restrict__ work_next,
+                  int two_ended, int sms, CostOrder co, unsigned *__restrict__ lazy_note,
+                  const Rec *__restrict__ rec_sorted, const Rec *__restrict__ rec, const unsigned *__restrict__ ids_sorted,
+                  const float *__restrict__ bg, float *__restrict__ out_color,
+                  float *__restrict__ out_depth, float *__restrict__ out_alpha, unsigned *__restrict__ n_contrib,
+                  float *__restrict__ final_T, ContribOut cw) {
+    render_fwd_body<1, 1, LAZY, true, true>(0, 0, 0, tile_order, order_ranges, n_tiles_nonempty, n_items, work_next, two_ended, sms, co, lazy_note, rec_sorted, rec, ids_sorted, bg, out_color, out_depth, out_alpha, n_contrib, final_T, &vt, cw);
+}
+
+// the fixed-point sums -> float32 (one thread per record); the max was raised in place
+constexpr int kContribFinalizeThreads = 256;
+__global__ void __launch_bounds__(kContribFinalizeThreads)
+contrib_finalize_kernel(long long n, const unsigned long long *__restrict__ sum_fx, float *__restrict__ weight_sum) {
+    const long long i = (long long)blockIdx.x * kContribFinalizeThreads + threadIdx.x;
+    if (i < n) weight_sum[i] = __fmul_rn(__ull2float_rn(__ldg(sum_fx + i)), kContribUnscale);
 }
 
 // ----------------------------------------------------------------------------------------------------------------

@@ -53,6 +53,26 @@ struct State {                       // what one forward leaves behind for its b
     int32_t staging = DGR_STAGING_SORTED;    // record staging the last stage-2 run chose (counts_host[3]): the backward's too
     int device = 0;
     DgrRasterOptions opt{0u};                // the forward's options: its backward takes the same
+    Tensor weight_sum, weight_max;           // contrib: the blending-weight statistics of the last stage-2 run, [P]
+};
+
+// DGR_RASTER_CONTRIB for the stage-2 render calls: the outputs [records] (shape `shape`) and their scratch, and the options that
+// carry them; without contrib, NULL options (the counterpart's call).
+struct ContribOut {
+    DgrContrib c{};
+    DgrRasterOptions opt{0u, nullptr, nullptr, nullptr};
+    Tensor weight_sum, weight_max, scratch;
+    ContribOut(bool contrib, at::IntArrayRef shape, const torch::TensorOptions &f32) {
+        if (!contrib) return;
+        weight_sum = torch::empty(shape, f32); weight_max = torch::empty(shape, f32);
+        const int64_t records = weight_sum.numel();
+        scratch = torch::empty({std::max<int64_t>((int64_t)dgr_contrib_scratch_bytes(records), 1)}, f32.dtype(torch::kUInt8));
+        c = DgrContrib{records ? weight_sum.data_ptr<float>() : nullptr, records ? weight_max.data_ptr<float>() : nullptr, scratch.data_ptr(),
+                       (uint64_t)scratch.numel()};
+        opt.flags = DGR_RASTER_CONTRIB;
+        opt.contrib = &c;
+    }
+    const DgrRasterOptions *options() const { return opt.flags ? &opt : nullptr; }
 };
 
 // scratch of the deterministic backward (dgr_*_backward_det), taken when torch.use_deterministic_algorithms(True) is in effect
@@ -82,7 +102,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<State>>
 forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modifier, int64_t sh_degree, bool prefiltered, bool debug,
         const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const OptTensor &sh,
         const OptTensor &colors, const Tensor &opac, const OptTensor &scales, const OptTensor &rots, const OptTensor &cov3D,
-        const OptTensor &sh_rest, bool activations, bool antialiasing) {
+        const OptTensor &sh_rest, bool activations, bool antialiasing, bool contrib) {
     auto st = std::make_shared<State>();
     st->opt.flags = antialiasing ? DGR_RASTER_ANTIALIAS : 0u;
     st->means3D = dev_f32(means3D, "means3D");
@@ -140,14 +160,20 @@ forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modif
     int64_t cap = hint.cap, n_inst = 0, n_big = 0;
     bool big = hint.big;
     int rerun = 0;
+    const ContribOut co(contrib, {P}, f32);                  // every stage-2 run rewrites it: the last run's values are kept
     while (true) {
         st->binning = torch::empty({(int64_t)dgr_binning_bytes((uint64_t)cap, (int32_t)H, (int32_t)W)}, u8);
         // ticket protocol: the scan kernel writes the counts and then the ticket into the pinned buffer; nothing but kernels
         // goes into the stream (programmatic dependent launches chain the whole forward) and the host polls the ticket
         const uint64_t ticket = ++so.ticket;
         volatile uint64_t *cnt = reinterpret_cast<volatile uint64_t *>(so.counts.data_ptr<int64_t>());
-        check(dgr_forward_render(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
-                                 (big ? DGR_FLAG_BIG_TILES : 0) | rerun, reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>()), ticket, nullptr, stream));
+        if (contrib)
+            check(dgr_forward_render_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
+                                        (big ? DGR_FLAG_BIG_TILES : 0) | rerun, reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>()), ticket,
+                                        nullptr, co.options(), stream));
+        else
+            check(dgr_forward_render(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
+                                     (big ? DGR_FLAG_BIG_TILES : 0) | rerun, reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>()), ticket, nullptr, stream));
         {
             pybind11::gil_scoped_release nogil;              // the wait for the early instance count
             uint64_t spins = 0;
@@ -169,6 +195,7 @@ forward(int64_t H, int64_t W, double tanfovx, double tanfovy, double scale_modif
     }
     { std::lock_guard<std::mutex> lk(g_mu); g_hints[key] = Hint{std::max<int64_t>((int64_t)(n_inst * 1.25) + 4096, 65536), n_big > 0}; }
     st->capacity = cap; st->n_inst = n_inst; st->staging = (int32_t)so.counts.data_ptr<int64_t>()[3];
+    st->weight_sum = co.weight_sum; st->weight_max = co.weight_max;
     return {color, st->radii, depth, alpha, st};
 }
 
@@ -253,6 +280,7 @@ struct ViewsState {
     int32_t staging = DGR_STAGING_SORTED;
     int device = 0;
     DgrRasterOptions opt{0u};
+    Tensor weight_sum, weight_max;   // contrib: [V,P]
 };
 
 std::unordered_map<uint64_t, Hint> g_views_hints;       // keyed by (device, P, H, W, V), apart from the single-view hints
@@ -287,7 +315,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
 views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double scale_modifier, int64_t sh_degree, bool debug,
                    const Tensor &tanfov, const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D,
                    const Tensor &sh, const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations,
-                   bool antialiasing) {
+                   bool antialiasing, bool contrib) {
     auto st = std::make_shared<ViewsState>();
     st->hw = hw;
     st->opt.flags = antialiasing ? DGR_RASTER_ANTIALIAS : 0u;
@@ -359,14 +387,22 @@ views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double 
     int64_t cap = hint.cap, n_inst = 0, n_big = 0;
     bool big = hint.big;
     int rerun = 0;
+    const ContribOut co(contrib, {V, P}, f32);
     while (true) {
         st->binning = torch::empty({(int64_t)dgr_views_binning_bytes((uint64_t)cap, (int32_t)V, (int32_t)H, (int32_t)W)}, u8);
         const uint64_t ticket = ++so.ticket;
         volatile uint64_t *cnt = reinterpret_cast<volatile uint64_t *>(so.counts.data_ptr<int64_t>());
         uint64_t *counts = reinterpret_cast<uint64_t *>(so.counts.data_ptr<int64_t>());
-        if (mixed)
+        if (mixed && contrib)
+            check(dgr_views_mixed_forward_render_ex(&st->s, ihw, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap,
+                                                    st->image.data_ptr(), &out, (big ? DGR_FLAG_BIG_TILES : 0) | rerun, counts, ticket, nullptr,
+                                                    co.options(), stream));
+        else if (mixed)
             check(dgr_views_mixed_forward_render(&st->s, ihw, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(),
                                                  &out, (big ? DGR_FLAG_BIG_TILES : 0) | rerun, counts, ticket, nullptr, stream));
+        else if (contrib)
+            check(dgr_views_forward_render_ex(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(),
+                                              &out, (big ? DGR_FLAG_BIG_TILES : 0) | rerun, counts, ticket, nullptr, co.options(), stream));
         else
             check(dgr_views_forward_render(&st->s, &st->g, st->geom.data_ptr(), st->binning.data_ptr(), (uint64_t)cap, st->image.data_ptr(), &out,
                                            (big ? DGR_FLAG_BIG_TILES : 0) | rerun, counts, ticket, nullptr, stream));
@@ -393,15 +429,16 @@ views_forward_impl(int64_t H, int64_t W, const std::vector<int32_t> &hw, double 
     { std::lock_guard<std::mutex> lk(g_mu);
       hints[key] = Hint{std::min<int64_t>(std::max<int64_t>((int64_t)(n_inst * 1.25) + 4096, 65536), 0xfffffffell), n_big > 0}; }
     st->capacity = cap; st->n_inst = n_inst; st->staging = (int32_t)so.counts.data_ptr<int64_t>()[3];
+    st->weight_sum = co.weight_sum; st->weight_max = co.weight_max;
     return {color, st->radii, depth, alpha, st};
 }
 
 std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
 views_forward(int64_t H, int64_t W, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov, const Tensor &bg,
               const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh, const Tensor &opac,
-              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations, bool antialiasing) {
+              const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations, bool antialiasing, bool contrib) {
     return views_forward_impl(H, W, {}, scale_modifier, sh_degree, debug, tanfov, bg, view, proj, campos, means3D, sh, opac, scales, rots,
-                              sh_rest, activations, antialiasing);
+                              sh_rest, activations, antialiasing, contrib);
 }
 
 // views of different sizes: image_hw = [V,2] (height, width); color [sum 3 H_v W_v], depth / alpha [sum H_v W_v] (flat)
@@ -409,12 +446,12 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, std::shared_ptr<ViewsState>>
 views_mixed_forward(const std::vector<int32_t> &image_hw, double scale_modifier, int64_t sh_degree, bool debug, const Tensor &tanfov,
                     const Tensor &bg, const Tensor &view, const Tensor &proj, const Tensor &campos, const Tensor &means3D, const Tensor &sh,
                     const Tensor &opac, const Tensor &scales, const Tensor &rots, const OptTensor &sh_rest, bool activations,
-                    bool antialiasing) {
+                    bool antialiasing, bool contrib) {
     TORCH_CHECK_VALUE(!image_hw.empty() && image_hw.size() % 2 == 0, "image_hw must have dimensions (num_views, 2)");
     int64_t H = 0, W = 0;                                    // the capacity ceiling's bytes per instance do not depend on the size
     for (size_t i = 0; i < image_hw.size(); i += 2) { H = std::max<int64_t>(H, image_hw[i]); W = std::max<int64_t>(W, image_hw[i + 1]); }
     return views_forward_impl(H, W, image_hw, scale_modifier, sh_degree, debug, tanfov, bg, view, proj, campos, means3D, sh, opac, scales,
-                              rots, sh_rest, activations, antialiasing);
+                              rots, sh_rest, activations, antialiasing, contrib);
 }
 
 // grads: (means3D, means2D [V,P,3], shs | features_dc, opacities, scales, rotations, features_rest); the per-Gaussian ones summed over views.
@@ -478,28 +515,35 @@ std::vector<Tensor> views_backward(const std::shared_ptr<ViewsState> &st, const 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     pybind11::class_<State, std::shared_ptr<State>>(m, "State")
         .def_readonly("capacity", &State::capacity)
-        .def_readonly("num_rendered", &State::n_inst);
+        .def_readonly("num_rendered", &State::n_inst)
+        .def_property_readonly("weight_sum", [](const State &s) { return s.weight_sum; })
+        .def_property_readonly("weight_max", [](const State &s) { return s.weight_max; });
     namespace py = pybind11;
     m.def("forward", &forward, "both forward stages through the C ABI (no arithmetic here)", py::arg("H"), py::arg("W"), py::arg("tanfovx"),
           py::arg("tanfovy"), py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("prefiltered"), py::arg("debug"), py::arg("bg"),
           py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"), py::arg("sh"), py::arg("colors"), py::arg("opac"),
-          py::arg("scales"), py::arg("rots"), py::arg("cov3D"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
+          py::arg("scales"), py::arg("rots"), py::arg("cov3D"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false,
+          py::arg("contrib") = false);
     m.def("backward", &backward, "backward through the C ABI", pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"),
           pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"),
           pybind11::arg("denom"), pybind11::arg("max_radii2D"), pybind11::arg("push_addr") = 0, pybind11::arg("camera") = false,
           pybind11::arg("absgrad") = pybind11::none());
     pybind11::class_<ViewsState, std::shared_ptr<ViewsState>>(m, "ViewsState")
         .def_readonly("capacity", &ViewsState::capacity)
-        .def_readonly("num_rendered", &ViewsState::n_inst);
+        .def_readonly("num_rendered", &ViewsState::n_inst)
+        .def_property_readonly("weight_sum", [](const ViewsState &s) { return s.weight_sum; })
+        .def_property_readonly("weight_max", [](const ViewsState &s) { return s.weight_max; });
     m.def("views_forward", &views_forward, "both forward stages of the batched-camera call through the C ABI", py::arg("H"), py::arg("W"),
           py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("debug"), py::arg("tanfov"), py::arg("bg"), py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"),
-          py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
+          py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false,
+          py::arg("contrib") = false);
     m.def("views_backward", &views_backward, "backward of the batched-camera call through the C ABI", pybind11::arg("state"),
           pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"), pybind11::arg("out"),
           pybind11::arg("camera") = false);
     m.def("views_mixed_forward", &views_mixed_forward, "both forward stages of the batched call with a size per view through the C ABI",
           py::arg("image_hw"), py::arg("scale_modifier"), py::arg("sh_degree"), py::arg("debug"), py::arg("tanfov"), py::arg("bg"), py::arg("view"), py::arg("proj"), py::arg("campos"), py::arg("means3D"),
-          py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false);
+          py::arg("sh"), py::arg("opac"), py::arg("scales"), py::arg("rots"), py::arg("sh_rest"), py::arg("activations"), py::arg("antialiasing") = false,
+          py::arg("contrib") = false);
     m.def("views_mixed_backward", &views_backward_impl, "backward of the batched call with a size per view through the C ABI",
           pybind11::arg("state"), pybind11::arg("grad_color"), pybind11::arg("grad_depth"), pybind11::arg("grad_alpha"), pybind11::arg("accumulate"),
           pybind11::arg("out"), pybind11::arg("xyz_gradient_accum"), pybind11::arg("denom"), pybind11::arg("max_radii2D"),

@@ -165,6 +165,53 @@ def _stream_ptr(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _contrib_opts(contrib, records, dev):
+    """The DgrRasterOptions argument of a stage-2 render *_ex call: None without contrib; with it, DGR_RASTER_CONTRIB and its
+    outputs -> (options pointer, (weight_sum, weight_max) float32 [records], the structs and scratch to keep alive)."""
+    if not contrib:
+        return None, None, None
+    lib = _lib.load()
+    ws = torch.empty((records,), dtype=torch.float32, device=dev)
+    wm = torch.empty((records,), dtype=torch.float32, device=dev)
+    scratch = torch.empty((max(1, lib.dgr_contrib_scratch_bytes(int(records))),), dtype=torch.uint8, device=dev)
+    c = _lib.DgrContrib(_ptr(ws) if records else None, _ptr(wm) if records else None, _ptr(scratch), scratch.numel())
+    opt = _lib.DgrRasterOptionsContrib(_lib.RASTER_CONTRIB, None, None, ctypes.pointer(c))
+    return ctypes.cast(ctypes.pointer(opt), ctypes.POINTER(_lib.DgrRasterOptions)), (ws, wm), (c, opt, scratch)
+
+
+class ContributionStats:
+    """Per-Gaussian blending-weight statistics accumulated over renders (DGR_RASTER_CONTRIB, include/dgr_b200.h): for every
+    rendered view, weight_sum adds the sum over the pixels where the Gaussian is composited of its weight w = alpha T, and
+    weight_max keeps the largest such w seen.  A Gaussian that no render composites (outside every view, or hidden behind
+    others) keeps weight_max == 0, whatever its radius; prune with GaussianModelB200.prune_by_contribution.
+    Pass it as contributions= to a render call: the forward updates it once per call (after its last stage-2 run, in view
+    order), under torch.no_grad too; the backward never touches it.  renders counts the views added."""
+
+    def __init__(self, P: int, device):
+        self.weight_sum = torch.zeros((P,), dtype=torch.float32, device=device)
+        self.weight_max = torch.zeros((P,), dtype=torch.float32, device=device)
+        self.renders = 0
+
+    def add(self, weight_sum, weight_max):
+        """Adds one render's ([P]) or one batch's ([V,P], view order) statistics."""
+        if weight_sum.dim() == 1:
+            weight_sum, weight_max = weight_sum.unsqueeze(0), weight_max.unsqueeze(0)
+        if weight_sum.shape[-1] != self.weight_sum.shape[0]:
+            raise ValueError("ContributionStats: %d Gaussians, the render has %d" % (self.weight_sum.shape[0], weight_sum.shape[-1]))
+        with torch.no_grad():
+            for v in range(weight_sum.shape[0]):
+                self.weight_sum.add_(weight_sum[v])
+                torch.maximum(self.weight_max, weight_max[v], out=self.weight_max)
+        self.renders += int(weight_sum.shape[0])
+
+
+def _add_contributions(contributions, state):
+    """After a forward that ran with contrib: its statistics into `contributions`, and out of the state."""
+    if contributions is not None:
+        contributions.add(*state.contrib)
+    state.contrib = None
+
+
 def _raster_opts(antialiasing):
     """The DgrRasterOptions argument of the *_ex calls."""
     return ctypes.byref(_lib.DgrRasterOptions(_lib.RASTER_ANTIALIAS if antialiasing else 0))
@@ -229,14 +276,16 @@ def _camera_input_grads(cams, needs, grads):
 class ForwardState:
     """Everything one forward leaves behind for its backward (upstream: ctx + geom/binning/img buffers)."""
     __slots__ = ("rs", "frame", "num_rendered", "capacity", "staging", "geom", "binning", "image", "radii", "alpha", "tensors",
-                 "fast", "stats_applied", "antialiasing")
+                 "fast", "stats_applied", "antialiasing", "contrib")
 
 
 def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, sh_rest=None, activations=False,
-                 antialiasing=False):
+                 antialiasing=False, contrib=False):
     """Runs both forward stages through the C ABI. Inputs are validated CUDA float32 tensors (or None).
     Returns (color, radii, depth, alpha, ForwardState).  antialiasing: the 2D Mip filter with opacity compensation
-    (DGR_RASTER_ANTIALIAS, include/dgr_b200.h); the state remembers it for the backward.
+    (DGR_RASTER_ANTIALIAS, include/dgr_b200.h); the state remembers it for the backward.  contrib: the render also leaves the
+    blending-weight statistics (DGR_RASTER_CONTRIB) of its last stage-2 run in state.contrib = (weight_sum, weight_max) [P]
+    (None without it).
 
     No host round trip sits between the kernels: the instance buffer is sized from a per-shape capacity hint, every
     kernel of the forward is enqueued, and only then does the host wait for the (early) instance-count event.  If the
@@ -245,9 +294,10 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
         color, radii, depth, alpha, cst = _FAST.forward(
             int(rs.image_height), int(rs.image_width), float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier), int(rs.sh_degree),
             bool(rs.prefiltered), bool(rs.debug), rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, means3D, sh, colors_precomp, opacities,
-            scales, rotations, cov3D, sh_rest, bool(activations), bool(antialiasing))
+            scales, rotations, cov3D, sh_rest, bool(activations), bool(antialiasing), bool(contrib))
         state = ForwardState()
         state.fast, state.rs, state.num_rendered, state.capacity = cst, rs, cst.num_rendered, cst.capacity
+        state.contrib = (cst.weight_sum, cst.weight_max) if contrib else None
         state.antialiasing = bool(antialiasing)
         state.radii, state.alpha = radii, None
         state.tensors = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, sh_rest)
@@ -272,11 +322,15 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
         key = (dev.index, P, H, W)
         cap, big = _CAPACITY_HINT.get(key, (max(65536, 16 * P), True))
         rerun = 0
+        copt, cout, _ckeep = _contrib_opts(contrib, P, dev)      # every stage-2 run rewrites it: the last run's values are kept
         while True:
             binning = torch.empty((lib.dgr_binning_bytes(cap, H, W),), **u8)
-            _lib.check(lib.dgr_forward_render(ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(geom), _ptr(binning),
-                                              ctypes.c_uint64(cap), _ptr(image), ctypes.byref(out), (1 if big else 0) | rerun,
-                                              ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event, st))
+            args = (ctypes.byref(fr.settings), ctypes.byref(fr.gaussians), _ptr(geom), _ptr(binning), ctypes.c_uint64(cap), _ptr(image),
+                    ctypes.byref(out), (1 if big else 0) | rerun, ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event)
+            if contrib:
+                _lib.check(lib.dgr_forward_render_ex(*args, copt, st))
+            else:
+                _lib.check(lib.dgr_forward_render(*args, st))
             _lib.check(lib.dgr_event_synchronize(event))
             n_inst, n_big = int(n_host[0]), int(n_host[1])
             if n_inst <= cap and (big or n_big == 0):
@@ -286,7 +340,7 @@ def forward_impl(rs, means3D, sh, colors_precomp, opacities, scales, rotations, 
             rerun = 2                                   # DGR_FLAG_RERUN
         _CAPACITY_HINT[key] = (max(int(n_inst * 1.25) + 4096, 65536), n_big > 0)
     state = ForwardState()
-    state.fast, state.antialiasing = None, bool(antialiasing)
+    state.fast, state.antialiasing, state.contrib = None, bool(antialiasing), cout
     state.rs, state.frame, state.num_rendered, state.capacity = rs, fr, n_inst, cap
     state.staging = int(n_host[3])                  # record staging of the last stage-2 run: its backward must use the same
     # alpha is a differentiable OUTPUT: storing it here would close the cycle state -> alpha -> grad_fn -> ctx -> state and leave
@@ -362,14 +416,15 @@ def _det_args(det, instances):
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
-                antialiasing=False, *cams):
+                antialiasing=False, contributions=None, *cams):
         ctx.cams = cams                  # (viewmatrix, projmatrix, campos) when their gradient is asked for (_camera_tensors)
         means3D = _dev_f32(means3D, "means3D")
         opacities = _dev_f32(opacities, "opacities")
         sh, colors_precomp = _opt(sh, "shs"), _opt(colors_precomp, "colors_precomp")
         scales, rotations, cov3D = _opt(scales, "scales"), _opt(rotations, "rotations"), _opt(cov3Ds_precomp, "cov3D_precomp")
         color, radii, depth, alpha, state = forward_impl(raster_settings, means3D, sh, colors_precomp, opacities, scales,
-                                                         rotations, cov3D, antialiasing=antialiasing)
+                                                         rotations, cov3D, antialiasing=antialiasing, contrib=contributions is not None)
+        _add_contributions(contributions, state)
         ctx.state = state
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -378,12 +433,12 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
         state = ctx.state
         cams = ctx.cams
-        cam_needed = any(ctx.needs_input_grad[10:])
+        cam_needed = any(ctx.needs_input_grad[11:])
         if state.fast is not None:
             g = _FAST.backward(state.fast, grad_color, grad_depth, grad_alpha, False, [], None, None, None,
                                camera=cam_needed)      # undefined -> None
-            cg = _camera_input_grads(cams, ctx.needs_input_grad[10:], g[9:12]) if cam_needed else [None] * len(cams)
-            return (g[0], g[1], g[2], g[3], g[4], g[5], g[6], g[7], None, None, *cg)
+            cg = _camera_input_grads(cams, ctx.needs_input_grad[11:], g[9:12]) if cam_needed else [None] * len(cams)
+            return (g[0], g[1], g[2], g[3], g[4], g[5], g[6], g[7], None, None, None, *cg)
         means3D, sh, colors_precomp, opacities, scales, rotations, cov3D, _ = state.tensors
         dev = means3D.device
         P, M = state.frame.P, state.frame.M
@@ -401,27 +456,30 @@ class _RasterizeGaussians(torch.autograd.Function):
         d_cov = torch.empty((P, 6), **f32) if cov3D is not None else None
         camera = _camera_outputs(0, dev) if cam_needed else None
         backward_impl(state, gC, gD, gA, d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, camera=camera)
-        cg = _camera_input_grads(cams, ctx.needs_input_grad[10:], camera) if cam_needed else [None] * len(cams)
+        cg = _camera_input_grads(cams, ctx.needs_input_grad[11:], camera) if cam_needed else [None] * len(cams)
         # ctx.state stays: a retain_graph backward runs again from the same buffers (they go away with the graph node)
-        return (d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, None, None, *cg)
+        return (d_means3D, d_means2D, d_sh, d_col, d_opac, d_scales, d_rot, d_cov, None, None, None, *cg)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
-                        antialiasing=False):
+                        antialiasing=False, contributions=None):
     """antialiasing=True: the 2D Mip filter with opacity compensation (Mip-Splatting), DGR_RASTER_ANTIALIAS of include/dgr_b200.h.
-    A viewmatrix / projmatrix / campos of raster_settings that requires grad receives its gradient (DGR_RASTER_CAMERA_GRADS)."""
+    A viewmatrix / projmatrix / campos of raster_settings that requires grad receives its gradient (DGR_RASTER_CAMERA_GRADS).
+    contributions (ContributionStats): the forward adds this render's blending-weight statistics to it (DGR_RASTER_CONTRIB)."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                     raster_settings, bool(antialiasing), *_camera_tensors([raster_settings]))
+                                     raster_settings, bool(antialiasing), contributions, *_camera_tensors([raster_settings]))
 
 
 class GaussianRasterizer(nn.Module):
     """Constructed per render call by the reference (gs_renderer.py:760): construction is trivial.  antialiasing=True renders
-    with the 2D Mip filter and opacity compensation (include/dgr_b200.h, DGR_RASTER_ANTIALIAS); the settings keep their 12 fields."""
+    with the 2D Mip filter and opacity compensation (include/dgr_b200.h, DGR_RASTER_ANTIALIAS); the settings keep their 12 fields.
+    contributions (ContributionStats): every forward adds its blending-weight statistics to it (DGR_RASTER_CONTRIB)."""
 
-    def __init__(self, raster_settings: GaussianRasterizationSettings, antialiasing: bool = False):
+    def __init__(self, raster_settings: GaussianRasterizationSettings, antialiasing: bool = False, contributions=None):
         super().__init__()
         self.raster_settings = raster_settings
         self.antialiasing = bool(antialiasing)
+        self.contributions = contributions
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -441,7 +499,7 @@ class GaussianRasterizer(nn.Module):
                 ((scales is not None or rotations is not None) and cov3D_precomp is not None):
             raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   self.raster_settings, self.antialiasing)
+                                   self.raster_settings, self.antialiasing, self.contributions)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -553,16 +611,17 @@ class _Views:
 class ViewsState:
     """Everything one batched forward leaves behind for its backward."""
     __slots__ = ("views", "capacity", "staging", "num_rendered", "geom", "binning", "image", "radii", "tensors", "fast", "mixed",
-                 "stats_applied", "antialiasing")
+                 "stats_applied", "antialiasing", "contrib")
 
 
 def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, sh_rest=None, activations=False, mixed=False,
-                       antialiasing=False):
+                       antialiasing=False, contrib=False):
     """Both forward stages of the batched call through the C ABI; inputs are validated CUDA float32 tensors.
     Returns (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W], ViewsState).  Same speculative-capacity
     protocol as forward_impl, with hints keyed by (device, P, H, W, V); the compiled host layer when it is loaded.
     mixed=True: every camera has its own image size (dgr_views_mixed_*); color [sum 3 H_v W_v], depth / alpha [sum H_v W_v]
-    are flat, view v's blocks one after the other, and the hints are keyed by (device, P, the sizes).  antialiasing: as forward_impl."""
+    are flat, view v's blocks one after the other, and the hints are keyed by (device, P, the sizes).  antialiasing: as forward_impl.
+    contrib: as forward_impl, state.contrib = (weight_sum, weight_max) [V,P]."""
     lib = _lib.load()
     dev = means3D.device
     if _FAST is not None:
@@ -573,12 +632,13 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
             hw = [int(x) for s in settings_list for x in (s.image_height, s.image_width)]
             color, radii, depth, alpha, cst = _FAST.views_mixed_forward(
                 hw, float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams, means3D, sh, opacities, scales, rotations, sh_rest,
-                bool(activations), bool(antialiasing))
+                bool(activations), bool(antialiasing), bool(contrib))
         else:
             color, radii, depth, alpha, cst = _FAST.views_forward(
                 int(s0.image_height), int(s0.image_width), float(s0.scale_modifier), int(s0.sh_degree), bool(s0.debug), *cams,
-                means3D, sh, opacities, scales, rotations, sh_rest, bool(activations), bool(antialiasing))
+                means3D, sh, opacities, scales, rotations, sh_rest, bool(activations), bool(antialiasing), bool(contrib))
         state = ViewsState()
+        state.contrib = (cst.weight_sum, cst.weight_max) if contrib else None
         state.fast, state.capacity, state.num_rendered, state.radii = cst, cst.capacity, cst.num_rendered, radii
         state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
         state.mixed, state.antialiasing = mixed, bool(antialiasing)
@@ -612,14 +672,19 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
         ceiling = _views_capacity_ceiling(lib, dev, V, H, W)
         cap, big = _CAPACITY_HINT.get(key, (min(max(65536, 16 * P * V), ceiling), True))
         rerun = 0
+        copt, cout, _ckeep = _contrib_opts(contrib, V * P, dev)
         while True:
             binning = torch.empty((lib.dgr_views_binning_bytes(cap, V, H, W),), **u8)
             args = (ctypes.byref(vw.gaussians), _ptr(geom), _ptr(binning), ctypes.c_uint64(cap), _ptr(image), ctypes.byref(out),
-                    (1 if big else 0) | rerun, ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event, st)
-            if mixed:
-                _lib.check(lib.dgr_views_mixed_forward_render(ctypes.byref(vw.settings), vw.hw, *args))
+                    (1 if big else 0) | rerun, ctypes.c_void_p(n_host.data_ptr()), ctypes.c_uint64(0), event)
+            if mixed and contrib:
+                _lib.check(lib.dgr_views_mixed_forward_render_ex(ctypes.byref(vw.settings), vw.hw, *args, copt, st))
+            elif mixed:
+                _lib.check(lib.dgr_views_mixed_forward_render(ctypes.byref(vw.settings), vw.hw, *args, st))
+            elif contrib:
+                _lib.check(lib.dgr_views_forward_render_ex(ctypes.byref(vw.settings), *args, copt, st))
             else:
-                _lib.check(lib.dgr_views_forward_render(ctypes.byref(vw.settings), *args))
+                _lib.check(lib.dgr_views_forward_render(ctypes.byref(vw.settings), *args, st))
             _lib.check(lib.dgr_event_synchronize(event))
             n_inst, n_big = int(n_host[0]), int(n_host[1])
             if n_inst <= cap and (big or n_big == 0):
@@ -632,6 +697,7 @@ def views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
         _CAPACITY_HINT[key] = (min(max(int(n_inst * 1.25) + 4096, 65536), _MAX_CAPACITY), n_big > 0)
     state = ViewsState()
     state.fast, state.mixed, state.antialiasing = None, mixed, bool(antialiasing)
+    state.contrib = (cout[0].view(V, P), cout[1].view(V, P)) if contrib else None
     state.views, state.capacity, state.staging, state.num_rendered = vw, cap, int(n_host[3]), n_inst
     state.geom, state.binning, state.image, state.radii = geom, binning, image, radii
     state.tensors = (means3D, sh, opacities, scales, rotations, sh_rest)
@@ -728,12 +794,13 @@ def _views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha, raw, f
 
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False, *cams):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False, contributions=None, *cams):
         ctx.cams = cams
         means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
         sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
         color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations,
-                                                               antialiasing=antialiasing)
+                                                               antialiasing=antialiasing, contrib=contributions is not None)
+        _add_contributions(contributions, state)
         ctx.state = state
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -741,23 +808,24 @@ class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
         (d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot), cg = _views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha,
-                                                                                                      False, 8)
+                                                                                                      False, 9)
         # ctx.state stays: a retain_graph backward runs again from the same buffers.  means2D may be None (no per-view gradient wanted)
-        return (d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None, *cg)
+        return (d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None, None, *cg)
 
 
-def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False):
+def rasterize_views(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False, contributions=None):
     """Renders ONE cloud from every camera of `settings_list` (GaussianRasterizationSettings, at most 64, all with the same
     image_height / image_width / sh_degree / scale_modifier) in one batched forward, and one batched backward.
     Returns (color [V,3,H,W], radii int32 [V,P], depth [V,1,H,W], alpha [V,1,H,W]); view v equals what GaussianRasterizer
     returns for camera v.  The gradients of means3D / shs / opacities / scales / rotations are summed over the views;
     means2D is [V,P,3] (e.g. zeros with requires_grad) or None: its gradient is per view, for densification.  SH colours and
     scale / rotation inputs only; no CPU path.  antialiasing: as GaussianRasterizer.  A camera tensor of a settings entry that
-    requires grad receives that view's own gradient (DGR_RASTER_CAMERA_GRADS)."""
+    requires grad receives that view's own gradient (DGR_RASTER_CAMERA_GRADS).  contributions (ContributionStats): the forward adds
+    every view's blending-weight statistics to it, in view order (DGR_RASTER_CONTRIB)."""
     settings_list = _check_views_settings(settings_list)
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
-    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list, bool(antialiasing),
+    return _RasterizeViews.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list, bool(antialiasing), contributions,
                                  *_camera_tensors(settings_list))
 
 
@@ -765,13 +833,15 @@ class GaussianViewsRasterizer(nn.Module):
     """`GaussianRasterizer` for a batch of same-size cameras: forward(means3D, means2D, opacities, shs, scales, rotations)
     -> (color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]), see rasterize_views."""
 
-    def __init__(self, settings_list, antialiasing=False):
+    def __init__(self, settings_list, antialiasing=False, contributions=None):
         super().__init__()
         self.settings_list = _check_views_settings(settings_list)
         self.antialiasing = bool(antialiasing)
+        self.contributions = contributions
 
     def forward(self, means3D, means2D, opacities, shs, scales, rotations):
-        return rasterize_views(self.settings_list, means3D, means2D, opacities, shs, scales, rotations, self.antialiasing)
+        return rasterize_views(self.settings_list, means3D, means2D, opacities, shs, scales, rotations, self.antialiasing,
+                               self.contributions)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -792,12 +862,13 @@ def split_views(settings_list, color, depth, alpha):
 
 class _RasterizeViewsMixed(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False, *cams):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, settings_list, antialiasing=False, contributions=None, *cams):
         ctx.cams = cams
         means3D, opacities = _dev_f32(means3D, "means3D"), _dev_f32(opacities, "opacities")
         sh, scales, rotations = _dev_f32(sh, "shs"), _dev_f32(scales, "scales"), _dev_f32(rotations, "rotations")
         color, radii, depth, alpha, state = views_forward_impl(settings_list, means3D, sh, opacities, scales, rotations, mixed=True,
-                                                               antialiasing=antialiasing)
+                                                               antialiasing=antialiasing, contrib=contributions is not None)
+        _add_contributions(contributions, state)
         ctx.state = state
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -805,20 +876,20 @@ class _RasterizeViewsMixed(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha):
         (d_means3D, d_means2D, d_sh, _, d_opac, d_scales, d_rot), cg = _views_backward_with_cameras(ctx, grad_color, grad_depth, grad_alpha,
-                                                                                                      False, 8)
-        return (d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None, *cg)
+                                                                                                      False, 9)
+        return (d_means3D, d_means2D if ctx.needs_input_grad[1] else None, d_sh, d_opac, d_scales, d_rot, None, None, None, *cg)
 
 
-def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False):
+def rasterize_views_mixed(settings_list, means3D, means2D, opacities, shs, scales, rotations, antialiasing=False, contributions=None):
     """rasterize_views for cameras of DIFFERENT image sizes (at most 64, one sh_degree / scale_modifier): one batched forward
     and one batched backward.  Returns (colors, radii, depths, alphas): colors a list of [3,H_v,W_v], depths / alphas lists of
     [1,H_v,W_v] (views of one flat tensor each), radii int32 [V,P]; view v equals what GaussianRasterizer returns for camera v.
     The gradients of means3D / shs / opacities / scales / rotations are summed over the views; means2D is [V,P,3] or None.
-    antialiasing: as GaussianRasterizer."""
+    antialiasing, contributions: as rasterize_views."""
     settings_list = _check_views_mixed_settings(settings_list)
     if means2D is not None and tuple(means2D.shape) != (len(settings_list), means3D.shape[0], 3):
         raise ValueError("means2D must have dimensions (num_views, num_points, 3)")
     color, radii, depth, alpha = _RasterizeViewsMixed.apply(means3D, means2D, shs, opacities, scales, rotations, settings_list,
-                                                            bool(antialiasing), *_camera_tensors(settings_list))
+                                                            bool(antialiasing), contributions, *_camera_tensors(settings_list))
     colors, depths, alphas = split_views(settings_list, color, depth, alpha)
     return colors, radii, depths, alphas

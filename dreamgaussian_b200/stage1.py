@@ -293,6 +293,19 @@ class GaussianModelB200:
     def prune(self, min_opacity, extent, max_screen_size):
         self.prune_points(self._prune_mask(min_opacity, extent, max_screen_size))
 
+    def prune_by_contribution(self, stats, min_weight_max):
+        """Removes the Gaussians whose largest blending weight over the renders in `stats` (rasterizer.ContributionStats) is below
+        min_weight_max: with a tiny threshold, those no render composited at all (outside every view or hidden behind others),
+        which the opacity prune keeps.  Through prune_points, so the Adam moments and densification statistics follow.
+        Returns how many were removed."""
+        wmax = stats.weight_max
+        if wmax.shape[0] != self.num_points:
+            raise ValueError("prune_by_contribution: the statistics have %d Gaussians, the model %d" % (wmax.shape[0], self.num_points))
+        mask = (wmax < min_weight_max).to(self.p["xyz"].device)
+        n = int(mask.sum())
+        self.prune_points(mask)
+        return n
+
     def reset_opacity(self):
         """gs_renderer.py:417-420 + replace_tensor_to_optimizer :464-477: opacity = inverse_sigmoid(min(sigmoid(o), 0.01)) and
         that group's Adam moments zeroed (torch keeps the group's step count: `stored_state["step"]` is left alone)."""
@@ -482,3 +495,24 @@ class Stage1Trainer:
         for _ in range(iters or self.cfg.iters):
             self.train_step()
         return torch.stack(self.losses).cpu().numpy()
+
+    # the 26 cameras the reference's save_model bakes the texture from (main.py:428-429): elevation, azimuth in degrees
+    EXPORT_VERS = [0] * 8 + [-45] * 8 + [45] * 8 + [-89.9, 89.9]
+    EXPORT_HORS = [0, 45, -45, 90, -90, 135, -135, 180] * 3 + [0, 0]
+
+    def export_settings(self, resolution=512):
+        """The export cameras at cfg.radius / cfg.fovy, resolution x resolution, white background."""
+        return [self._settings(v, h, self.cfg.radius, resolution, (1.0, 1.0, 1.0)) for v, h in zip(self.EXPORT_VERS, self.EXPORT_HORS)]
+
+    def prune_unseen(self, min_weight_max, resolution=512):
+        """Before extracting the mesh or saving the PLY: renders the 26 export cameras in one batched forward (no gradients) with
+        the blending-weight statistics and removes the Gaussians whose largest weight in any of them is below min_weight_max
+        (GaussianModelB200.prune_by_contribution).  Returns how many were removed.  train() does not call it."""
+        from .fused import rasterize_views_raw
+        from .rasterizer import ContributionStats
+        g = self.gaussians
+        stats = ContributionStats(g.num_points, self.device)
+        with torch.no_grad():
+            rasterize_views_raw(self.export_settings(resolution), g._xyz, None, g._features_dc, g._features_rest, g._opacity, g._scaling,
+                                g._rotation, antialiasing=self.cfg.antialiasing, contributions=stats)
+        return g.prune_by_contribution(stats, min_weight_max)

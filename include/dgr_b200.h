@@ -354,11 +354,54 @@ size_t dgr_camera_grad_scratch_bytes(int32_t V, int32_t P);
  * thread per Gaussian after the per-Gaussian backward (absgrad_stats); DESIGN.md §4 has the times.  Densify with
  * dgr_densify_plan_ex. */
 #define DGR_RASTER_ABS_GRAD 16u
+/* == Per-Gaussian blending-weight statistics (DGR_RASTER_CONTRIB, stage-2 render *_ex calls only) ==
+ * For one render of view v and record r (r = g for the single-view call, r = v P + g for the batched calls), over exactly the
+ * pixels p where the forward composites the record (power <= 0, alpha >= 1/255, before the T < 1e-4 stop), with the blending
+ * weight w_p = alpha_p T_p, alpha_p = min(0.99, o G_p) (o = o_eff with DGR_RASTER_ANTIALIAS, the opacity the record carries):
+ *   weight_sum[r] = sum_p w_p          weight_max[r] = max_p w_p
+ * Both are 0 for a record with radius 0 and for one that is never composited (hidden behind others, or behind the T stop).
+ * In exact arithmetic sum_r weight_sum[r] over a view's records equals the sum of that view's alpha image.
+ * Outputs: device float32 [records]; DgrContrib.scratch: device memory of at least dgr_contrib_scratch_bytes(records) bytes.
+ * Each call zeroes its outputs and scratch before its render and writes them completely, so a stage-2 re-run (DGR_FLAG_RERUN)
+ * leaves the last run's values; nothing is accumulated here (a caller adds renders up after the run it keeps).
+ * Deterministic by construction: each render warp reduces its (tile, sub-tile) item's weights of a record in a fixed order, the
+ * item partials are added as 64-bit fixed point with scale 2^38 (integer atomics, so the order the items arrive in does not
+ * matter) and the max is an atomicMax on the bits of a non-negative float.  Bound: an image has at most 51200 tiles of 256 pixels
+ * and w <= 0.99, so a record's sum is below 2^24 and its fixed-point total below 2^62; a partial is rounded to the nearest 2^-38
+ * (absolute), and the total to float32 once.  The outputs are bit-identical from call to call, whatever dgr_set_tuning's knobs
+ * and the record staging, and a view of a batched call gives what the single-view call of that camera gives.
+ * With the bit, the forward render runs its default sub-tile shape (<1,1>: 8x4 pixels per warp, one hit at a time) as the
+ * render_*_fwd_contrib kernels, whatever the pixels-per-lane and hits-together knobs say, followed by contrib_finalize (one
+ * thread per record); images, depth, alpha, radii and the forward state a backward reads are those of the call without the bit.
+ * Accepted by dgr_forward_render_ex, dgr_views_forward_render_ex and dgr_views_mixed_forward_render_ex (flags NULL / 0: exactly
+ * the counterpart's call).  Refused before any device work, each with its own dgr_last_error text: any other bit on those calls,
+ * the bit on a preprocess or backward *_ex call, contrib == NULL, a NULL output or scratch, and a scratch below
+ * dgr_contrib_scratch_bytes.  Bits 2u and 8u stay unknown (refused), and `contrib` is read only with the bit, so a
+ * DgrRasterOptions that ends before it is never read past its end. */
+#define DGR_RASTER_CONTRIB 32u
+typedef struct DgrContrib {
+    float *weight_sum;       /* [records] */
+    float *weight_max;       /* [records] */
+    void *scratch;           /* device, >= dgr_contrib_scratch_bytes(records) */
+    uint64_t scratch_bytes;
+} DgrContrib;
+size_t dgr_contrib_scratch_bytes(int64_t records);
 typedef struct DgrRasterOptions {
     uint32_t flags;          /* DGR_RASTER_* bits */
     const DgrCameraGrads *camera;   /* read only when flags has DGR_RASTER_CAMERA_GRADS */
     float *xyz_gradient_accum_abs;  /* [P], read only when flags has DGR_RASTER_ABS_GRAD */
+    const DgrContrib *contrib;      /* read only when flags has DGR_RASTER_CONTRIB */
 } DgrRasterOptions;
+int dgr_forward_render_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, void *binning,
+                          uint64_t capacity_instances, void *image, const DgrImages *out, int32_t flags,
+                          uint64_t *counts_host, uint64_t ticket, void *count_ready_event, const DgrRasterOptions *opt, void *stream);
+int dgr_views_forward_render_ex(const DgrViews *s, const DgrGaussians *g, void *geom, void *binning, uint64_t capacity_instances,
+                                void *image, const DgrImages *out, int32_t flags, uint64_t *counts_host, uint64_t ticket,
+                                void *count_ready_event, const DgrRasterOptions *opt, void *stream);
+int dgr_views_mixed_forward_render_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom, void *binning,
+                                      uint64_t capacity_instances, void *image, const DgrImages *out, int32_t flags,
+                                      uint64_t *counts_host, uint64_t ticket, void *count_ready_event, const DgrRasterOptions *opt,
+                                      void *stream);
 int dgr_forward_preprocess_ex(const DgrSettings *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii,
                               const DgrRasterOptions *opt, void *stream);
 int dgr_views_forward_preprocess_ex(const DgrViews *s, const DgrGaussians *g, void *geom, void *image, int32_t *radii,
