@@ -289,6 +289,20 @@ def trained_mix(seed=0, W=512, H=512, deg=3):
     return settings_of(cam, deg), as_inputs({k: v[perm] for k, v in g.items()})
 
 
+def compact_mix(P, seed=0, W=72, H=56, deg=1):
+    """Exactly P Gaussians drawn (in random order) from a small mix of the regimes above: ordinary, saturated (no pairs,
+    trained_mix's band), needles with axis ratios 10-30 (the ratios test_trained_regimes_gpu.py holds to the suite's rules),
+    clamped colours, and near-plane / frustum-edge Gaussians.  tests/test_kernel_coverage_gpu.py builds its scenes with it."""
+    cam, rng = camera(W, H), np.random.default_rng(seed)
+    g = concat(_background(cam, rng, P // 2, deg), _saturated(cam, rng, P // 3, deg, pairs=False, band=0.05),
+               _needles(cam, rng, P // 12, deg, constructed=0, log_ratio=(1.0, np.log10(30.0))), _dark(cam, rng, P // 8, deg),
+               _frustum_edge(cam, rng, P // 16, max(2, P // 80), deg))
+    n = g["means3D"].shape[0]
+    assert n >= P, (n, P)
+    idx = rng.permutation(n)[:P]
+    return settings_of(cam, deg), as_inputs({k: v[idx] for k, v in g.items()})
+
+
 def raw_of(inputs, seed=0, extremes=False):
     """scene.to_raw_parameters of the inputs; extremes: on disjoint 2% slices, opacity logits in +-12, log-scales moved to
     within +-6 of the cloud's mean on Gaussians with axis ratios below 3 (one shift per Gaussian), and quaternion lengths from 1e-3 to 1e3."""
