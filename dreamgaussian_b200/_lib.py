@@ -272,6 +272,44 @@ def load():
     return lib
 
 
+MCMC_EXPORTS = ("dgr_mcmc_last_error", "dgr_mcmc_relocation", "dgr_mcmc_scratch_bytes", "dgr_mcmc_refine", "dgr_mcmc_inject_noise")
+_mcmc = None
+
+
+def load_mcmc():
+    """Load libdgr_mcmc.so (include/dgr_mcmc.h: the opt-in MCMC densification), building it first when its sources are newer.
+    Raises on failure: there is no other implementation of these entry points."""
+    global _mcmc
+    if _mcmc is not None:
+        return _mcmc
+    path = _build.MCMC_LIB_PATH
+    if _build.mcmc_is_stale():
+        try:
+            _build.build_mcmc()
+        except Exception as e:  # noqa: BLE001
+            if not os.path.exists(path):
+                raise RuntimeError("libdgr_mcmc.so is not built and could not be compiled here (%s). "
+                                   "Run `python -m dreamgaussian_b200.build` on a machine with nvcc." % e)
+    lib = ctypes.CDLL(path)
+    vp, i32 = ctypes.c_void_p, ctypes.c_int32
+    lib.dgr_mcmc_last_error.restype = ctypes.c_char_p
+    lib.dgr_mcmc_relocation.restype = ctypes.c_int
+    lib.dgr_mcmc_relocation.argtypes = [i32, vp, vp, vp, vp, vp, vp]
+    lib.dgr_mcmc_scratch_bytes.restype = ctypes.c_size_t
+    lib.dgr_mcmc_scratch_bytes.argtypes = [i32, i32]
+    lib.dgr_mcmc_refine.restype = ctypes.c_int
+    lib.dgr_mcmc_refine.argtypes = [i32, i32, ctypes.POINTER(DgrDensifyTensors), vp, vp, ctypes.c_float, vp, ctypes.c_size_t, vp, vp]
+    lib.dgr_mcmc_inject_noise.restype = ctypes.c_int
+    lib.dgr_mcmc_inject_noise.argtypes = [i32, vp, vp, vp, vp, vp, ctypes.c_float, vp]
+    _mcmc = lib
+    return lib
+
+
+def check_mcmc(code):
+    if code != 0:
+        raise RuntimeError("libdgr_mcmc: %s (code %d)" % (load_mcmc().dgr_mcmc_last_error().decode(), code))
+
+
 def profile_collect(max_records=4096):
     """-> list of (kernel name, milliseconds) recorded since dgr_profile_enable(1)."""
     lib = load()

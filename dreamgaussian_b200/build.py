@@ -92,6 +92,52 @@ def build(force=False, verbose=False):
     return LIB_PATH
 
 
+# ---- the opt-in MCMC densification (csrc/mcmc/, include/dgr_mcmc.h): a library of its own, so the rasterizer library and its
+# kernel set stay what they are
+MCMC_DIR = os.path.join(CSRC, "mcmc")
+MCMC_LIB_PATH = os.path.join(LIB_DIR, "libdgr_mcmc.so")
+MCMC_HASH_PATH = os.path.join(LIB_DIR, "libdgr_mcmc.srchash")
+
+
+def mcmc_sources():
+    return sorted(os.path.join(MCMC_DIR, f) for f in os.listdir(MCMC_DIR) if f.endswith((".cu", ".cuh"))) + [
+        os.path.join(HERE, "..", "include", n) for n in ("dgr_mcmc.h", "dgr_b200.h", "dgr_constants.h")]
+
+
+def _mcmc_hash():
+    import hashlib
+    h = hashlib.sha256(" ".join(NVCC_FLAGS).encode())
+    for s in mcmc_sources():
+        with open(s, "rb") as f:
+            h.update(os.path.basename(s).encode() + b"\0" + f.read())
+    return h.hexdigest()
+
+
+def mcmc_is_stale():
+    if not os.path.exists(MCMC_LIB_PATH) or not os.path.exists(MCMC_HASH_PATH):
+        return True
+    with open(MCMC_HASH_PATH) as f:
+        return f.read().strip() != _mcmc_hash()
+
+
+def build_mcmc(force=False):
+    """Compile dreamgaussian_b200/csrc/mcmc/dgr_mcmc_api.cu -> dreamgaussian_b200/lib/libdgr_mcmc.so (sm_90a). Returns the path."""
+    if not force and not mcmc_is_stale():
+        return MCMC_LIB_PATH
+    os.makedirs(LIB_DIR, exist_ok=True)
+    cmd = [_nvcc()] + NVCC_FLAGS + ["-o", MCMC_LIB_PATH, os.path.join(MCMC_DIR, "dgr_mcmc_api.cu")]
+    if os.path.exists("/usr/bin/g++"):
+        cmd += ["-ccbin", "/usr/bin/g++"]
+    proc = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    with open(os.path.join(LIB_DIR, "build_mcmc.log"), "w") as f:
+        f.write(" ".join(cmd) + "\n" + proc.stdout)
+    if proc.returncode != 0:
+        raise RuntimeError("nvcc failed on the MCMC library:\n" + proc.stdout[-8000:])
+    with open(MCMC_HASH_PATH, "w") as f:
+        f.write(_mcmc_hash())
+    return MCMC_LIB_PATH
+
+
 # ---- the compiled PyTorch host layer over the C ABI (csrc/dgr_torch.cpp): g++ only, links libdgr_b200.so
 HOST_PATH = os.path.join(LIB_DIR, "dgr_torch_host.so")
 HOST_HASH = os.path.join(LIB_DIR, "dgr_torch_host.srchash")
@@ -137,3 +183,4 @@ def build_host(force=False):
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose=True))
     print(build_host(force="--force" in sys.argv))
+    print(build_mcmc(force="--force" in sys.argv))

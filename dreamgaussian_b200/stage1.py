@@ -58,6 +58,67 @@ class OptimConfig(NamedTuple):
 
 GROUPS = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
 
+# MCMC densification: include/dgr_constants.h DGR_MCMC_* (tests/test_mcmc_cpu.py holds the two equal)
+MCMC_N_MAX = 51
+MCMC_MIN_OPACITY = 0.005
+MCMC_OPACITY_MAX = 1.0 - 2.0 ** -23
+MCMC_GROW_PERCENT = 105
+MCMC_NOISE_K, MCMC_NOISE_X0 = 100.0, 0.995
+MCMC_NOISE_LR = 5e5
+MCMC_OPACITY_REG = MCMC_SCALE_REG = 0.01
+
+
+def mcmc_add_count(P, cap_max):
+    """Rows one MCMC refinement appends: max(0, min(cap_max, floor(1.05 P)) - P)."""
+    return max(0, min(int(cap_max), P * MCMC_GROW_PERCENT // 100) - P)
+
+
+def mcmc_relocation(opacity, scale, ratio):
+    """The relocation formula alone on activated values (gsplat's `relocation` op), one launch of dgr_mcmc_relocation (float64
+    inside): n = ratio clamped to [1, 51], o' = 1 - (1 - o)^(1/n), s' = s o / D with D = sum_{m=1..n} C(n,m) (-1)^(m-1) o'^m / sqrt(m)
+    (1 where D = 0); no clamp.  opacity [K] (or [K,1]), scale [K,3] float32 and ratio [K] integer CUDA tensors -> (o' shaped like
+    opacity, s' [K,3])."""
+    if not (opacity.is_cuda and scale.is_cuda and ratio.is_cuda):
+        raise ValueError("mcmc_relocation: CUDA tensors expected (the formula runs in dgr_mcmc_relocation)")
+    K = opacity.numel()
+    if tuple(scale.shape) != (K, 3) or ratio.numel() != K:
+        raise ValueError("mcmc_relocation: opacity [K], scale [K,3], ratio [K]")
+    op = opacity.detach().float().contiguous()
+    sc = scale.detach().float().contiguous()
+    r = ratio.to(torch.int32).contiguous()
+    new_op, new_sc = torch.empty_like(op), torch.empty_like(sc)
+    lib = _lib.load_mcmc()
+    with torch.cuda.device(op.device):
+        st = ctypes.c_void_p(torch.cuda.current_stream(op.device).cuda_stream)
+        _lib.check_mcmc(lib.dgr_mcmc_relocation(K, op.data_ptr(), sc.data_ptr(), r.data_ptr(), new_op.data_ptr(), new_sc.data_ptr(), st))
+    return new_op, new_sc
+
+
+def _mcmc_relocate(o, n):
+    """(o', o / D) in float64, the operation order of csrc/dgr_mcmc.cuh::mcmc_relocate (terms past m = n are +-0)."""
+    o_new = -torch.expm1(torch.log1p(-o) / n)
+    c, p, D = torch.ones_like(o), torch.ones_like(o), torch.zeros_like(o)
+    nd = n.double()
+    for m in range(1, MCMC_N_MAX + 1):
+        c = c * (nd - m + 1) / m
+        p = p * o_new
+        t = c * p / math.sqrt(m)
+        D = D + t if m & 1 else D - t
+    return o_new, torch.where(D > 0, o / D, torch.ones_like(o))
+
+
+def _mcmc_opacity(raw):
+    """sigmoid in float64 rounded once to float32: the weights the kernels compute."""
+    return torch.sigmoid(raw.double()).float()
+
+
+def _mcmc_update(op_raw, sc_raw, picks, min_opacity):
+    """Raw opacity / scaling of rows picked `picks` times: logit(clamp(o', min_opacity, 1 - 2^-23)), scaling + log(o / D)."""
+    o = _mcmc_opacity(op_raw).double()
+    o_new, factor = _mcmc_relocate(o, (picks.to(torch.int64) + 1).clamp(max=MCMC_N_MAX))
+    oc = o_new.clamp(min_opacity, MCMC_OPACITY_MAX)
+    return torch.log(oc / (1 - oc)).float(), (sc_raw.double() + torch.log(factor)[:, None]).float()
+
 
 def build_rotation(r):
     """gs_renderer.py:85-107 (normalises the quaternion)."""
@@ -293,6 +354,124 @@ class GaussianModelB200:
     def prune(self, min_opacity, extent, max_screen_size):
         self.prune_points(self._prune_mask(min_opacity, extent, max_screen_size))
 
+    # ---- MCMC densification (Kheradmand et al., NeurIPS 2024): relocate dead rows, grow to a cap, position noise
+    def relocate_and_grow_mcmc(self, cap_max, min_opacity=MCMC_MIN_OPACITY, u_relocate=None, u_add=None):
+        """One MCMC refinement of the P rows: relocation of the rows with sigmoid(opacity) <= min_opacity onto live rows drawn in
+        proportion to their opacity, then growth by n_add = max(0, min(cap_max, floor(1.05 P)) - P) rows drawn from all rows in
+        proportion to their opacity (include/dgr_mcmc.h dgr_mcmc_refine has the rule).  Sources get the relocation formula and zero
+        Adam moments; relocated dead rows keep their own moments (as the published code); appended rows get zero moments.  Nothing is
+        pruned.  u_relocate [P] / u_add [n_add]: uniform draws in [0, 1), by default from `noise_gen`.  With `fused_densify` on CUDA
+        it runs the kernels (no host synchronisation), otherwise the torch restatement.  Returns the number of relocated rows as a
+        device int32 scalar."""
+        P, dev = self.num_points, self.p["xyz"].device
+        n_add = mcmc_add_count(P, cap_max)
+        min_opacity = float(np.float32(min_opacity))
+        gen = getattr(self, "noise_gen", None)
+        if u_relocate is None:
+            u_relocate = torch.rand((P,), device=dev, generator=gen)
+        if u_add is None:
+            u_add = torch.rand((n_add,), device=dev, generator=gen)
+        u_relocate, u_add = u_relocate.to(dev, torch.float32).contiguous(), u_add.to(dev, torch.float32).contiguous()
+        if u_relocate.shape != (P,) or u_add.shape != (n_add,):
+            raise ValueError("relocate_and_grow_mcmc: u_relocate must be [%d] and u_add [%d]" % (P, n_add))
+        with torch.no_grad():
+            if getattr(self, "fused_densify", False) and self.p["xyz"].is_cuda and P > 0:
+                n = self._mcmc_refine_fused(n_add, u_relocate, u_add, min_opacity)
+            else:
+                n = self._mcmc_refine_torch(n_add, u_relocate, u_add, min_opacity)
+        self._reset_stats()
+        return n
+
+    def _mcmc_refine_fused(self, n_add, u_relocate, u_add, min_opacity):
+        lib = _lib.load_mcmc()
+        P, dev = self.num_points, self.p["xyz"].device
+        with torch.cuda.device(dev):
+            st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            nbytes = lib.dgr_mcmc_scratch_bytes(P, n_add)
+            scratch = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+            n_relocated = torch.zeros((), dtype=torch.int32, device=dev)
+            t = _lib.DgrDensifyTensors()
+            new_p, new_m, new_v = {}, {}, {}
+            for i, k in enumerate(GROUPS):
+                src = self.p[k].detach()
+                new_p[k] = torch.empty((P + n_add,) + tuple(src.shape[1:]), dtype=torch.float32, device=dev)
+                new_m[k], new_v[k] = torch.empty_like(new_p[k]), torch.empty_like(new_p[k])
+                t.inp[i], t.exp_avg_in[i], t.exp_avg_sq_in[i] = src.data_ptr(), self.exp_avg[k].data_ptr(), self.exp_avg_sq[k].data_ptr()
+                t.out[i], t.exp_avg_out[i], t.exp_avg_sq_out[i] = new_p[k].data_ptr(), new_m[k].data_ptr(), new_v[k].data_ptr()
+                t.width[i] = int(np.prod(src.shape[1:]))
+            _lib.check_mcmc(lib.dgr_mcmc_refine(P, n_add, ctypes.byref(t), u_relocate.data_ptr(), u_add.data_ptr() if n_add else None,
+                                           min_opacity, scratch.data_ptr(), nbytes, n_relocated.data_ptr(), st))
+            self.p = {k: v.requires_grad_(True) for k, v in new_p.items()}
+            self.exp_avg, self.exp_avg_sq = new_m, new_v
+        return n_relocated
+
+    def _mcmc_refine_torch(self, n_add, u_relocate, u_add, min_opacity):
+        """The rule of dgr_mcmc_refine with torch ops: searchsorted on a float64 cumsum, then tensor indexing (what the GPU tests hold the kernels to)."""
+        P, dev = self.num_points, self.p["xyz"].device
+        out = {k: v.detach().clone() for k, v in self.p.items()}
+        m = {k: v.clone() for k, v in self.exp_avg.items()}
+        v = {k: x.clone() for k, x in self.exp_avg_sq.items()}
+        n_relocated = torch.zeros((), dtype=torch.int32, device=dev)
+        if P > 0:
+            o = _mcmc_opacity(out["opacity"][:, 0])
+            dead = o <= min_opacity
+            C = torch.cumsum(torch.where(dead, torch.zeros_like(o), o).double(), 0)
+            dead_idx = dead.nonzero()[:, 0]
+            if float(C[-1]) > 0 and dead_idx.numel() > 0:
+                src = torch.searchsorted(C, u_relocate[:dead_idx.numel()].double() * C[-1], right=True)
+                src = torch.where(src >= P, (~dead).nonzero()[-1, 0], src)
+                picks = torch.bincount(src, minlength=P)
+                rows = (picks > 0).nonzero()[:, 0]
+                out["opacity"][rows, 0], out["scaling"][rows] = _mcmc_update(out["opacity"][rows, 0], out["scaling"][rows], picks[rows],
+                                                                             min_opacity)
+                for k in GROUPS:
+                    out[k][dead_idx] = out[k][src]
+                    m[k][rows] = 0
+                    v[k][rows] = 0
+                n_relocated.fill_(dead_idx.numel())
+            if n_add > 0:
+                C = torch.cumsum(_mcmc_opacity(out["opacity"][:, 0]).double(), 0)
+                src = torch.searchsorted(C, u_add.double() * C[-1], right=True).clamp(max=P - 1)
+                picks = torch.bincount(src, minlength=P)
+                rows = (picks > 0).nonzero()[:, 0]
+                out["opacity"][rows, 0], out["scaling"][rows] = _mcmc_update(out["opacity"][rows, 0], out["scaling"][rows], picks[rows],
+                                                                             min_opacity)
+                for k in GROUPS:
+                    m[k][rows] = 0
+                    v[k][rows] = 0
+                    out[k] = torch.cat((out[k], out[k][src]), 0)
+                    m[k] = torch.cat((m[k], torch.zeros_like(out[k][P:])), 0)
+                    v[k] = torch.cat((v[k], torch.zeros_like(out[k][P:])), 0)
+        self.p = {k: x.contiguous().requires_grad_(True) for k, x in out.items()}
+        self.exp_avg = {k: x.contiguous() for k, x in m.items()}
+        self.exp_avg_sq = {k: x.contiguous() for k, x in v.items()}
+        return n_relocated
+
+    def inject_noise_mcmc(self, scale, normals=None):
+        """xyz += scale g(o) R diag(s^2) R^T z in place, g(o) = 1 / (1 + exp(-100 ((1 - o) - 0.995))) (near-transparent Gaussians
+        move, opaque ones do not); scale = lr_xyz(step) * noise_lr in the published rule.  normals [P,3]: standard normals, by default
+        from `noise_gen`.  With `fused_densify` on CUDA one launch (dgr_mcmc_inject_noise), otherwise torch ops."""
+        P, dev = self.num_points, self.p["xyz"].device
+        if normals is None:
+            normals = torch.randn((P, 3), device=dev, generator=getattr(self, "noise_gen", None))
+        normals = normals.to(dev, torch.float32).contiguous()
+        if normals.shape != (P, 3):
+            raise ValueError("inject_noise_mcmc: normals must be [%d, 3]" % P)
+        with torch.no_grad():
+            if getattr(self, "fused_densify", False) and self.p["xyz"].is_cuda and P > 0:
+                lib = _lib.load_mcmc()
+                with torch.cuda.device(dev):
+                    st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+                    _lib.check_mcmc(lib.dgr_mcmc_inject_noise(P, self.p["xyz"].data_ptr(), self.p["opacity"].data_ptr(), self.p["scaling"].data_ptr(),
+                                                         self.p["rotation"].data_ptr(), normals.data_ptr(), float(scale), st))
+                return
+            o = torch.sigmoid(self.p["opacity"].detach())
+            gate = 1.0 / (1.0 + torch.exp(-MCMC_NOISE_K * ((1 - o) - MCMC_NOISE_X0)))
+            R = build_rotation(self.p["rotation"].detach())
+            s2 = torch.exp(self.p["scaling"].detach()) ** 2
+            a = torch.bmm(R.transpose(1, 2), normals[:, :, None])[:, :, 0] * s2 * (scale * gate)
+            self.p["xyz"].add_(torch.bmm(R, a[:, :, None])[:, :, 0])
+
     def prune_by_contribution(self, stats, min_weight_max):
         """Removes the Gaussians whose largest blending weight over the renders in `stats` (rasterizer.ContributionStats) is below
         min_weight_max: with a tiny threshold, those no render composited at all (outside every view or hidden behind others),
@@ -341,6 +520,16 @@ class Stage1Config(NamedTuple):
     # AbsGS densification: split by the absolute-gradient statistic at this threshold (clone as before); None = the default loop.
     # Needs fused=True: the statistic exists only inside the backward render.
     densify_abs_grad_threshold: Optional[float] = None
+    # "mcmc": 3DGS-MCMC's rule instead of clone / split / prune — relocate dead Gaussians and grow by 5 % per refinement up to
+    # mcmc_cap_max (in the density window at the densification interval), position noise every step, the two regularisers in the loss,
+    # no opacity reset.  The cap's default is about the count the default loop reaches in 500 iterations; nobody has measured it
+    # for quality.
+    densify_strategy: str = "default"
+    mcmc_cap_max: int = 43000
+    mcmc_noise_lr: float = MCMC_NOISE_LR
+    mcmc_opacity_reg: float = MCMC_OPACITY_REG
+    mcmc_scale_reg: float = MCMC_SCALE_REG
+    mcmc_min_opacity: float = MCMC_MIN_OPACITY
 
 
 class GuidanceStub:
@@ -382,7 +571,13 @@ class Stage1Trainer:
         if cfg.densify_abs_grad_threshold is not None and not fused:
             raise ValueError("Stage1Trainer: densify_abs_grad_threshold needs fused=True (the reference formulation takes its statistics "
                              "from means2D.grad, which has no per-pixel absolute values)")
+        if cfg.densify_strategy not in ("default", "mcmc"):
+            raise ValueError("Stage1Trainer: densify_strategy must be 'default' or 'mcmc', not %r" % (cfg.densify_strategy,))
+        if cfg.densify_strategy == "mcmc" and cfg.densify_abs_grad_threshold is not None:
+            raise ValueError("Stage1Trainer: densify_strategy='mcmc' does not split by a gradient statistic; "
+                             "densify_abs_grad_threshold must be None")
         self.cfg, self.device, self.fused, self.batched = cfg, torch.device(device), fused, batched
+        self.mcmc = cfg.densify_strategy == "mcmc"
         self.rng = np.random.default_rng(cfg.seed)
         self.scene = scene
         cloud = scene.make_cloud(cfg.num_pts, cfg.sh_degree, seed=cfg.seed, anisotropic=False, sigma=1.0)      # positions only
@@ -433,13 +628,20 @@ class Stage1Trainer:
         g.update_learning_rate(self.step)
         g.zero_grad()
         densify_window = cfg.density_start_iter <= self.step <= cfg.density_end_iter
+        track = densify_window and not self.mcmc          # the MCMC rule needs no densification statistics
         if self.batched:
-            loss = self._batched_loss(step_ratio, densify_window)
+            loss = self._batched_loss(step_ratio, track)
         else:
-            loss = self._loss(step_ratio, densify_window)
+            loss = self._loss(step_ratio, track)
+        if self.mcmc:
+            loss = loss + cfg.mcmc_opacity_reg * torch.sigmoid(g._opacity).mean() + cfg.mcmc_scale_reg * torch.exp(g._scaling).mean()
         loss.backward()
         g.optimizer_step()
-        if densify_window:
+        if self.mcmc:
+            if densify_window and self.step % cfg.densification_interval == 0:
+                g.relocate_and_grow_mcmc(cfg.mcmc_cap_max, cfg.mcmc_min_opacity)
+            g.inject_noise_mcmc(g.lr["xyz"] * cfg.mcmc_noise_lr)
+        elif densify_window:
             if not self.fused:          # the reference's three torch updates (main.py:279-281, gs_renderer.py:625-627)
                 with torch.no_grad():
                     vis, radii, st = self._last["visibility_filter"], self._last["radii"], g.stats

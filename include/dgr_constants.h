@@ -25,6 +25,17 @@
 #define DGR_SH_OFFSET       0.5f        /* gs_renderer.py:793                                                 */
 #define DGR_AA_RATIO_FLOOR  2.5e-5f     /* UNVERIFIED-EXT anti-aliased mode: floor under det(cov2D) / det(cov2D + lowpass) */
 
+/* MCMC densification (Kheradmand et al., NeurIPS 2024; gsplat MCMCStrategy), recalled from the published code */
+#define DGR_MCMC_N_MAX         51       /* UNVERIFIED-EXT size of the published binomial table: copies per source clamp here   */
+#define DGR_MCMC_MIN_OPACITY   0.005f   /* UNVERIFIED-EXT dead at or below this opacity; floor of the relocated opacity        */
+#define DGR_MCMC_OPACITY_MAX   (1.0 - 1.0 / 8388608.0) /* UNVERIFIED-EXT 1 - 2^-23: ceiling of the relocated opacity        */
+#define DGR_MCMC_GROW_PERCENT  105      /* UNVERIFIED-EXT target count floor(1.05 P) per refinement, up to the cap             */
+#define DGR_MCMC_NOISE_K       100.0f   /* UNVERIFIED-EXT noise gate 1 / (1 + exp(-k ((1 - o) - x0)))                          */
+#define DGR_MCMC_NOISE_X0      0.995f   /* UNVERIFIED-EXT                                                                      */
+#define DGR_MCMC_NOISE_LR      5e5f     /* UNVERIFIED-EXT noise scale = lr_xyz(step) * noise_lr                                */
+#define DGR_MCMC_OPACITY_REG   0.01f    /* UNVERIFIED-EXT loss += opacity_reg * mean(sigmoid(opacity))                         */
+#define DGR_MCMC_SCALE_REG     0.01f    /* UNVERIFIED-EXT loss += scale_reg * mean(exp(scaling))                               */
+
 /* sh_utils.py:26-43 */
 #define DGR_SH_C0   0.28209479177387814f
 #define DGR_SH_C1   0.4886025119029199f
