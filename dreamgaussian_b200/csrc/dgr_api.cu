@@ -12,6 +12,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -326,23 +327,34 @@ void launch_camera_bwd(int V, const ViewTable &vt, float2 tan0, const float *tan
              g->shs, g->shs_rest, g->scales, g->rotations, g->cov3D_precomp, radii, touched, grad_rec, rows);
 }
 
-#define DGR_DISPATCH(FN, ...)                                                                              \
-    do {                                                                                                   \
-        const bool sh_ = g->shs != nullptr, cov_ = g->cov3D_precomp != nullptr;                            \
-        if (g->activations) switch (s->sh_degree) {       /* raw parameters: SH + scale/rotation only */     \
-            case 0: FN<0, true, false, true>(__VA_ARGS__); break;                                           \
-            case 1: FN<1, true, false, true>(__VA_ARGS__); break;                                           \
-            case 2: FN<2, true, false, true>(__VA_ARGS__); break;                                           \
-            default: FN<3, true, false, true>(__VA_ARGS__); break;                                          \
-        }                                                                                                  \
-        else if (!sh_) { if (cov_) FN<0, false, true, false>(__VA_ARGS__); else FN<0, false, false, false>(__VA_ARGS__); } \
-        else switch (s->sh_degree) {                                                                       \
-            case 0: if (cov_) FN<0, true, true, false>(__VA_ARGS__); else FN<0, true, false, false>(__VA_ARGS__); break;  \
-            case 1: if (cov_) FN<1, true, true, false>(__VA_ARGS__); else FN<1, true, false, false>(__VA_ARGS__); break;  \
-            case 2: if (cov_) FN<2, true, true, false>(__VA_ARGS__); else FN<2, true, false, false>(__VA_ARGS__); break;  \
-            default: if (cov_) FN<3, true, true, false>(__VA_ARGS__); else FN<3, true, false, false>(__VA_ARGS__); break; \
-        }                                                                                                  \
-    } while (0)
+// The compile-time configuration of the per-Gaussian kernels, handed to a generic lambda as integral constants.
+template <int N> using IntC = std::integral_constant<int, N>;
+// fn(DEG) for a checked SH degree 0..3
+template <class Fn>
+void with_sh_degree(int sh_degree, Fn &&fn) {
+    switch (sh_degree) {
+        case 0: fn(IntC<0>{}); break;
+        case 1: fn(IntC<1>{}); break;
+        case 2: fn(IntC<2>{}); break;
+        default: fn(IntC<3>{}); break;
+    }
+}
+// fn(DEG, HAS_SH, HAS_COV, RAW) of a checked call's inputs
+template <class Fn>
+void dispatch_gaussians(int sh_degree, const DgrGaussians *g, Fn &&fn) {
+    using T = std::true_type;
+    using F = std::false_type;
+    if (g->activations) with_sh_degree(sh_degree, [&](auto deg) { fn(deg, T{}, F{}, T{}); });   // raw parameters: SH + scale/rotation only
+    else if (!g->shs) { if (g->cov3D_precomp) fn(IntC<0>{}, F{}, T{}, F{}); else fn(IntC<0>{}, F{}, F{}, F{}); }
+    else if (g->cov3D_precomp) with_sh_degree(sh_degree, [&](auto deg) { fn(deg, T{}, T{}, F{}); });
+    else with_sh_degree(sh_degree, [&](auto deg) { fn(deg, T{}, F{}, F{}); });
+}
+// fn(DEG, RAW) of the batched call (SH + scale / rotation inputs only)
+template <class Fn>
+void dispatch_views(int sh_degree, bool raw, Fn &&fn) {
+    if (raw) with_sh_degree(sh_degree, [&](auto deg) { fn(deg, std::true_type{}); });
+    else with_sh_degree(sh_degree, [&](auto deg) { fn(deg, std::false_type{}); });
+}
 
 // The two camera-gradient kernels after the per-Gaussian backward of a checked call (S = DgrSettings or DgrViews).  tanfov = NULL:
 // single view, tan0 = (tanfovx, tanfovy).  An empty cloud launches only the reduction, which writes zeros.
@@ -352,8 +364,10 @@ int camera_grads(const S *s, const DgrGaussians *g, const DgrCameraGrads *cam, i
     float *rows = reinterpret_cast<float *>(cam->scratch);
     const int nblk = (g->P + kPreThreads - 1) / kPreThreads;
     if (g->P > 0)
-        DGR_KERNEL("camera_bwd", st, s->debug, DGR_DISPATCH(launch_camera_bwd, V, vt, tan0, tanfov, s->scale_modifier, s->viewmatrix,
-                                                            s->projmatrix, s->campos, g, radii, touched, grad_rec, rows, aa, st));
+        DGR_KERNEL("camera_bwd", st, s->debug, dispatch_gaussians(s->sh_degree, g, [&](auto deg, auto sh, auto cov, auto raw) {
+            launch_camera_bwd<deg, sh, cov, raw>(V, vt, tan0, tanfov, s->scale_modifier, s->viewmatrix, s->projmatrix, s->campos, g, radii,
+                                                 touched, grad_rec, rows, aa, st);
+        }));
     DGR_KERNEL("camera_reduce", st, s->debug, launch_k(camera_reduce_kernel, dim3((unsigned)V), dim3(kCamReduceThreads), 0, st, false, nblk,
                                                       (const float *)rows, cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos));
     return 0;
@@ -434,6 +448,19 @@ int persistent_grid(DevInfo *d, K kernel, int threads, size_t smem) {
     return g;
 }
 
+// Launch of a persistent render kernel: its persistent grid, at most max_ctas CTAs (its work items over the warps of a CTA, or the
+// tiles of the deterministic backward) and, when the knob cta is set, at most that many CTAs per SM.
+template <class K, class... Args>
+int launch_persistent(DevInfo *dv, K kernel, const char *name, int threads, size_t smem, int max_ctas, const std::atomic<int> &cta, bool pdl,
+                      int debug, cudaStream_t st, const Args &...args) {
+    int grid = min(persistent_grid(dv, kernel, threads, smem), max_ctas);
+    if (cta.load() > 0) grid = min(grid, cta.load() * dv->sms);
+    DGR_KERNEL(name, st, debug, launch_k(kernel, dim3((unsigned)grid), dim3(threads), smem, st, pdl, args...));
+    return 0;
+}
+// work items of a render kernel with ppl pixels per lane: its warps' sub-tiles of every 16x16 tile
+constexpr int sub_tiles(int ppl) { return ppl == 4 ? SubTile<4>::kPerTile : ppl == 2 ? SubTile<2>::kPerTile : SubTile<1>::kPerTile; }
+
 // ---- launch steps shared by the single-view and the batched (dgr_views_*) entry points ---------------------------------------
 // A forward re-run with corrected capacity guesses repeats everything from instance emission on: the per-tile totals and run
 // matrix are still valid, what the first, clipped render pass filed as backward costs is not.
@@ -511,10 +538,13 @@ int check_det(const DetArgs &d, const DgrGaussianGrads *gout, uint64_t capacity,
 }
 
 // Everything between the backward's memset and its per-Gaussian kernel: masked counts -> exclusive scan (goff) -> render_bwd_det ->
-// det_moments_gather, which leaves grad_rec as the default render kernel would, summed in a fixed order.  vt = NULL: single view.
-int det_render(DevInfo *dv, const DetArgs &d, long long R, int H, int W, int gx, const ViewTable *vt, int tiles, const char *image,
-               const ImageLayout &IL, char *geom, const GeomLayout &GL, const char *binning, const BinningLayout &BL, bool lazy,
-               const float *bg, const DgrImageGrads *gin, float *grad_rec, bool abs, int debug, cudaStream_t st) {
+// det_moments_gather, which leaves grad_rec as the default render kernel would, summed in a fixed order.  head: the render kernel's
+// leading arguments, (H, W, gx) of a single view or (vt) of a batch.
+template <class... Head>
+int det_render(DevInfo *dv, const DetArgs &d, long long R, int tiles, const char *image, const ImageLayout &IL, char *geom,
+               const GeomLayout &GL, const char *binning, const BinningLayout &BL, bool lazy, const float *bg, const DgrImageGrads *gin,
+               float *grad_rec, bool abs, int debug, cudaStream_t st, const Head &...head) {
+    constexpr bool views = sizeof...(Head) == 1;
     if (debug) {                                     // debug: the caller's instance count against the forward's own (a host sync)
         unsigned long long n_fwd = 0;
         DGR_CUDA(cudaMemcpyAsync(&n_fwd, geom + offsetof(GeomHeader, n_inst), sizeof(n_fwd), cudaMemcpyDeviceToHost, st));
@@ -550,26 +580,20 @@ int det_render(DevInfo *dv, const DetArgs &d, long long R, int H, int W, int gx,
     const unsigned *nc = reinterpret_cast<const unsigned *>(image + IL.off_ncontrib);
     const unsigned long long n_slots = d.instances;
     const size_t smem = sizeof(DetSmem);
-    auto launch = [&](auto kernel, const char *name, auto... head) -> int {
-        int grid = min(persistent_grid(dv, kernel, kDetThreads, smem), tiles);
-        if (g_cta_bwd.load() > 0) grid = min(grid, g_cta_bwd.load() * dv->sms);
-        DGR_KERNEL(name, st, debug, launch_k(kernel, dim3((unsigned)grid), dim3(kDetThreads), smem, st, true, head..., order, oranges,
-                                             &work->n_nonempty, bwd_next, recs, rec, ids, (const unsigned *)goff, n_slots, bg, fT, nc,
-                                             gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, mom));
-        return 0;
+    auto launch = [&](auto kernel, const char *name) {
+        return launch_persistent(dv, kernel, name, kDetThreads, smem, tiles, g_cta_bwd, true, debug, st, head..., order, oranges,
+                                 &work->n_nonempty, bwd_next, recs, rec, ids, (const unsigned *)goff, n_slots, bg, fT, nc, gin->dL_dcolor,
+                                 gin->dL_ddepth, gin->dL_dalpha, mom);
     };
     int e = 0;
     if (d.instances == 0) {}                         // nothing binned: no instance row to fill (the gather flags any touched record)
-    else if (abs) {
-        if (vt) e = lazy ? launch(render_views_bwd_det_abs_kernel<true>, "render_views_bwd_det_abs", *vt)
-                         : launch(render_views_bwd_det_abs_kernel<false>, "render_views_bwd_det_abs", *vt);
-        else e = lazy ? launch(render_bwd_det_abs_kernel<true>, "render_bwd_det_abs", H, W, gx)
-                      : launch(render_bwd_det_abs_kernel<false>, "render_bwd_det_abs", H, W, gx);
+    else if constexpr (views) {
+        if (abs) e = launch(lazy ? render_views_bwd_det_abs_kernel<true> : render_views_bwd_det_abs_kernel<false>, "render_views_bwd_det_abs");
+        else e = launch(lazy ? render_views_bwd_det_kernel<true> : render_views_bwd_det_kernel<false>, "render_views_bwd_det");
+    } else {
+        if (abs) e = launch(lazy ? render_bwd_det_abs_kernel<true> : render_bwd_det_abs_kernel<false>, "render_bwd_det_abs");
+        else e = launch(lazy ? render_bwd_det_kernel<true> : render_bwd_det_kernel<false>, "render_bwd_det");
     }
-    else if (vt) e = lazy ? launch(render_views_bwd_det_kernel<true>, "render_views_bwd_det", *vt)
-                     : launch(render_views_bwd_det_kernel<false>, "render_views_bwd_det", *vt);
-    else e = lazy ? launch(render_bwd_det_kernel<true>, "render_bwd_det", H, W, gx)
-                  : launch(render_bwd_det_kernel<false>, "render_bwd_det", H, W, gx);
     if (e) return e;
     if (abs)
         DGR_KERNEL("det_moments_gather_abs", st, debug, launch_k(det_moments_gather_abs_kernel, dim3(nb), dim3(256), 0, st, true, R, touched,
@@ -577,6 +601,113 @@ int det_render(DevInfo *dv, const DetArgs &d, long long R, int H, int W, int gx,
     else
         DGR_KERNEL("det_moments_gather", st, debug, launch_k(det_moments_gather_kernel, dim3(nb), dim3(256), 0, st, true, R, touched,
                                                              (const unsigned *)goff, (const float *)mom, n_slots, grad_rec));
+    return 0;
+}
+
+// ---- the stages shared by the single-view and the batched entry points after their checks -----------------------------------
+// head: the leading arguments of the render kernels, (H, W, gx) of a single view or (vt) of a batch; the rest of each render
+// kernel family's argument list is written once, below.
+
+// Stage 2 of a forward (instance emission -> per-tile sorts -> render) of P Gaussians and `records` records.  emit(launch) launches
+// the emit kernel as launch(kernel, name, its leading arguments); pick(fwd, lazy) launches the render kernel the knobs select as
+// fwd(kernel, name, ppl[, ContribOut]).  cost_ppl: the backward sub-tile shape the render files its costs for.
+template <class S, class Emit, class Pick, class... Head>
+int forward_stage2(const S *s, int P, int64_t records, char *geom, const GeomLayout &GL, char *image, const ImageLayout &IL, char *binning,
+                   uint64_t capacity, int32_t flags, uint64_t *counts_host, uint64_t ticket, void *count_ready_event, const DgrImages *out,
+                   const DgrContrib *cb, int cost_ppl, cudaStream_t st, Emit &&emit, Pick &&pick, const Head &...head) {
+    const BinningLayout BL(capacity);
+    const int tiles = GL.tiles;
+    const Rec *rec = reinterpret_cast<const Rec *>(geom + GL.off_rec);
+    unsigned long long *keys = binning ? reinterpret_cast<unsigned long long *>(binning + BL.off_keys) : nullptr;
+    unsigned *ids = binning ? reinterpret_cast<unsigned *>(binning + BL.off_ids) : nullptr;
+    Rec *recs = binning ? reinterpret_cast<Rec *>(binning + BL.off_rec) : nullptr;
+    unsigned *tile_order = reinterpret_cast<unsigned *>(image + IL.off_order);
+    uint2 *oranges = reinterpret_cast<uint2 *>(image + IL.off_oranges);
+    TileWork *work = reinterpret_cast<TileWork *>(image + IL.off_work);
+    DevInfo *dv = dev_info();
+    if (!dv) return -1;
+    if (flags & DGR_FLAG_RERUN)
+        if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
+    if (int e = contrib_clear(cb, records, st)) return e;
+    // instance emission; its extra block publishes ranges / order / counts (capacity 0: only that block has work to do)
+    const int nb = (P > 0 && capacity > 0) ? GL.nblocks : 0;
+    auto launch_emit = [&](auto kernel, const char *name, const auto &...emit_head) -> int {
+        DGR_KERNEL(name, st, s->debug,
+                   launch_k(kernel, dim3(nb + 1), dim3(kPreThreads), (size_t)tiles * 4, st, !(flags & DGR_FLAG_RERUN), emit_head..., GL.iters, nb,
+                            rec, reinterpret_cast<const unsigned *>(geom + GL.off_touched), reinterpret_cast<const unsigned *>(image + IL.off_count),
+                            (unsigned long long)capacity, reinterpret_cast<const unsigned *>(geom + GL.off_runs), keys,
+                            reinterpret_cast<uint2 *>(image + IL.off_ranges), reinterpret_cast<GeomHeader *>(geom), tile_order, oranges, work,
+                            reinterpret_cast<unsigned *>(image + IL.off_biglist), (volatile unsigned long long *)(ticket ? counts_host : nullptr),
+                            (unsigned long long)ticket));
+        return 0;
+    };
+    if (int e = emit(launch_emit)) return e;
+    if (int e = copy_counts(geom, counts_host, ticket, count_ready_event, st)) return e;
+    const bool lazy = stage_records_by_id(capacity, dv, counts_host);
+    if (P > 0 && capacity > 0)
+        if (int e = launch_tile_sorts(dv, image, IL, tiles, flags & DGR_FLAG_BIG_TILES, lazy, keys, rec, ids, recs, s->debug, st)) return e;
+    // persistent forward render: every (tile, sub-tile) is a work item, handed out heaviest tile first
+    const CostOrder co = cost_order(image, IL, tiles, cost_ppl);
+    auto fwd = [&](auto kernel, const char *name, int ppl, const auto &...contrib) {
+        const int items = tiles * sub_tiles(ppl);
+        return launch_persistent(dv, kernel, name, kRenderThreads, 0, (items + kRenderWarps - 1) / kRenderWarps, g_cta_fwd, true, s->debug, st,
+                                 head..., tile_order, oranges, &work->n_nonempty, (unsigned)items, &work->fwd_next, g_two_ended.load(), dv->sms,
+                                 co, &work->lazy, recs, rec, ids, s->bg, out->color, out->depth, out->alpha,
+                                 reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT), contrib...);
+    };
+    if (int e = pick(fwd, lazy)) return e;
+    return contrib_finalize(cb, records, s->debug, st);
+}
+
+// A backward of P Gaussians in V views (view table vt, tangents tan0 or tanfov as camera_grads takes them) from its memset on: the
+// render (the deterministic one with det), the per-Gaussian backward, the AbsGS statistic of stats_views and the camera gradients.
+// pick(bwd, lazy) launches the render kernel the knobs select as bwd(kernel, name, ppl); pre_bwd(touched, grad_rec, aa) launches
+// the per-Gaussian backward.
+template <class S, class Pick, class PreBwd, class... Head>
+int backward_stages(const S *s, const DgrGaussians *g, int V, const ViewTable &vt, float2 tan0, const float *tanfov, uint64_t stats_views,
+                    char *geom, const GeomLayout &GL, const char *image, const ImageLayout &IL, const char *binning, uint64_t capacity,
+                    int32_t staging, const int32_t *radii, const DgrImageGrads *gin, const DetArgs *det, uint32_t flags,
+                    const DgrCameraGrads *cam, float *abs_accum, cudaStream_t st, Pick &&pick, PreBwd &&pre_bwd, const Head &...head) {
+    const long long records = (long long)g->P * V;
+    const int tiles = GL.tiles;
+    float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
+    // one memset: the work counter of the persistent backward render kernel + the per-Gaussian moment accumulators
+    DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)records * kGradRecFloats * 4, st));
+    if (binning && capacity > 0) {
+        DevInfo *dv = dev_info();
+        if (!dv) return -1;
+        const BinningLayout BL(capacity);
+        // the record staging the forward chose (dgr_forward_render): only then does the sorted copy exist
+        const bool lazy = staging == DGR_STAGING_BY_ID;
+        if (det) {
+            if (int e = det_render(dv, *det, records, tiles, image, IL, geom, GL, binning, BL, lazy, s->bg, gin, grad_rec, abs_accum != nullptr,
+                                   s->debug, st, head...)) return e;
+        } else {
+            const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
+            // ppl 1 or 2: the backward's 8x4 or 8x8 sub-tiles; the work order is the one the forward grouped its costs in for that
+            // shape (the kernel checks it)
+            auto bwd = [&](auto kernel, const char *name, int ppl) {
+                const size_t smem = (ppl == 1 ? sizeof(BwdSmem<1>) : sizeof(BwdSmem<2>)) * kRenderWarps;
+                const int items = tiles * sub_tiles(ppl);
+                return launch_persistent(dv, kernel, name, kRenderThreads, smem, (items + kRenderWarps - 1) / kRenderWarps, g_cta_bwd, false,
+                                         s->debug, st, head..., reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty,
+                                         reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork), g_two_ended.load(), dv->sms,
+                                         cost_order(image, IL, tiles, ppl), reinterpret_cast<const uint2 *>(image + IL.off_oranges),
+                                         reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec),
+                                         &work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids), s->bg,
+                                         reinterpret_cast<const float *>(image + IL.off_finalT),
+                                         reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth,
+                                         gin->dL_dalpha, grad_rec);
+            };
+            if (int e = pick(bwd, lazy)) return e;
+        }
+    }
+    const unsigned *touched = reinterpret_cast<const unsigned *>(geom + GL.off_touched);
+    const bool aa = flags & DGR_RASTER_ANTIALIAS;
+    if (int e = pre_bwd(touched, grad_rec, aa)) return e;
+    if (abs_accum)
+        if (int e = absgrad_stats(g->P, V, vt, stats_views, radii, grad_rec, abs_accum, s->debug, st)) return e;
+    if (cam) return camera_grads(s, g, cam, V, vt, tan0, tanfov, radii, touched, grad_rec, aa, st);
     return 0;
 }
 }  // namespace
@@ -655,7 +786,9 @@ static int forward_preprocess(const DgrSettings *s, const DgrGaussians *g, void 
     const bool aa = flags & DGR_RASTER_ANTIALIAS;
     if (g->P > 0) {
         if (!radii) return fail(-1, "radii is NULL");
-        DGR_KERNEL("preprocess_fwd", st, s->debug, DGR_DISPATCH(launch_pre_fwd, s, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), aa, st));
+        DGR_KERNEL("preprocess_fwd", st, s->debug, dispatch_gaussians(s->sh_degree, g, [&](auto deg, auto sh, auto cov, auto raw) {
+            launch_pre_fwd<deg, sh, cov, raw>(s, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), aa, st);
+        }));
     }
     return 0;
 }
@@ -688,79 +821,23 @@ static int forward_render(const DgrSettings *s, const DgrGaussians *g, void *geo
     const int H = s->image_height, W = s->image_width;
     GeomLayout GL(g->P, H, W);
     ImageLayout IL(H, W);
-    BinningLayout BL(capacity);
     const int tiles = IL.gx * IL.gy;
     if ((size_t)tiles * 4 > kMaxTileSmem) return fail(-3, "image has more than 51200 tiles (16x16): not supported");
-    uint2 *ranges = reinterpret_cast<uint2 *>(image + IL.off_ranges);
-    unsigned *tile_count = reinterpret_cast<unsigned *>(image + IL.off_count);
-    const unsigned *run_matrix = reinterpret_cast<const unsigned *>(geom + GL.off_runs);
-    unsigned *n_contrib = reinterpret_cast<unsigned *>(image + IL.off_ncontrib);
-    float *final_T = reinterpret_cast<float *>(image + IL.off_finalT);
-    GeomHeader *hdr = reinterpret_cast<GeomHeader *>(geom);
-    const Rec *rec = reinterpret_cast<const Rec *>(geom + GL.off_rec);
-    unsigned long long *keys = binning ? reinterpret_cast<unsigned long long *>(binning + BL.off_keys) : nullptr;
-    unsigned *ids = binning ? reinterpret_cast<unsigned *>(binning + BL.off_ids) : nullptr;
-    Rec *recs = binning ? reinterpret_cast<Rec *>(binning + BL.off_rec) : nullptr;
-
-    unsigned *tile_order = reinterpret_cast<unsigned *>(image + IL.off_order);
-    unsigned *big_list = reinterpret_cast<unsigned *>(image + IL.off_biglist);
-    TileWork *work = reinterpret_cast<TileWork *>(image + IL.off_work);
-    DevInfo *dv = dev_info();
-    if (!dv) return -1;
-    if (flags & DGR_FLAG_RERUN)
-        if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
-    if (int e = contrib_clear(cb, g->P, st)) return e;
-    {
-        // instance emission; its extra block publishes ranges / order / counts (capacity 0: only that block has work to do)
-        const size_t smem = (size_t)tiles * 4;
-        const int nb = (g->P > 0 && capacity > 0) ? GL.nblocks : 0;
-        DGR_KERNEL("emit_instances", st, s->debug,
-                   launch_k(emit_instances_kernel, dim3(nb + 1), dim3(kPreThreads), smem, st, !(flags & DGR_FLAG_RERUN), g->P, IL.gx, tiles, GL.iters, nb, rec,
-                            reinterpret_cast<const unsigned *>(geom + GL.off_touched), (const unsigned *)tile_count, (unsigned long long)capacity,
-                            run_matrix, keys, ranges, hdr, tile_order, reinterpret_cast<uint2 *>(image + IL.off_oranges), work, big_list,
-                            (volatile unsigned long long *)(ticket ? counts_host : nullptr), (unsigned long long)ticket));
-    }
-    if (int e = copy_counts(geom, counts_host, ticket, count_ready_event, st)) return e;
-    const bool lazy = stage_records_by_id(capacity, dv, counts_host);
-    if (g->P > 0 && capacity > 0)
-        if (int e = launch_tile_sorts(dv, image, IL, tiles, flags & DGR_FLAG_BIG_TILES, lazy, keys, rec, ids, recs, s->debug, st)) return e;
-    // persistent forward render: every (tile, sub-tile) is a work item, handed out heaviest tile first
-    const int ppl = g_ppl_fwd.load(), uf = g_u_fwd.load();
-    const CostOrder co = cost_order(image, IL, tiles, g_ppl_bwd.load());
-#define DGR_RENDER_FWD_L(PPL_, U_, L_)                                                                          \
-    do {                                                                                                        \
-        const int items_ = tiles * SubTile<PPL_>::kPerTile;                                                     \
-        int grid_ = min(persistent_grid(dv, render_fwd_kernel<PPL_, U_, L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
-        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                               \
-        DGR_KERNEL("render_fwd", st, s->debug,                                                                  \
-                   launch_k(render_fwd_kernel<PPL_, U_, L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, H, W, IL.gx,   \
-                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),         \
-                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
-                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids,                                      \
-                            s->bg, out->color, out->depth, out->alpha, n_contrib, final_T));                     \
-    } while (0)
-#define DGR_RENDER_FWD(PPL_, U_) do { if (lazy) DGR_RENDER_FWD_L(PPL_, U_, true); else DGR_RENDER_FWD_L(PPL_, U_, false); } while (0)
-    // DGR_RASTER_CONTRIB: the default shape's statistics variant, whatever the knobs
-#define DGR_RENDER_FWD_C(L_)                                                                                    \
-    do {                                                                                                        \
-        const int items_ = tiles * SubTile<1>::kPerTile;                                                        \
-        int grid_ = min(persistent_grid(dv, render_fwd_contrib_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
-        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                               \
-        DGR_KERNEL("render_fwd_contrib", st, s->debug,                                                          \
-                   launch_k(render_fwd_contrib_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, H, W, IL.gx, \
-                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),         \
-                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
-                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids,                                      \
-                            s->bg, out->color, out->depth, out->alpha, n_contrib, final_T, contrib_out(cb)));    \
-    } while (0)
-    if (cb) { if (lazy) DGR_RENDER_FWD_C(true); else DGR_RENDER_FWD_C(false); }
-    else if (ppl == 4) DGR_RENDER_FWD(4, 1);
-    else if (ppl == 2) DGR_RENDER_FWD(2, 2);
-    else { if (uf == 4) DGR_RENDER_FWD(1, 4); else DGR_RENDER_FWD(1, 1); }      // default <1,1>: 58 registers, 8 CTAs per SM, no spill
-#undef DGR_RENDER_FWD_L
-#undef DGR_RENDER_FWD
-#undef DGR_RENDER_FWD_C
-    return contrib_finalize(cb, g->P, s->debug, st);
+    return forward_stage2(s, g->P, g->P, geom, GL, image, IL, binning, capacity, flags, counts_host, ticket, count_ready_event, out, cb,
+                          g_ppl_bwd.load(), st,
+                          [&](auto emit) { return emit(emit_instances_kernel, "emit_instances", g->P, IL.gx, tiles); },
+                          [&](auto fwd, bool lazy) {
+                              // DGR_RASTER_CONTRIB: the default shape's statistics variant, whatever the knobs
+                              if (cb) return fwd(lazy ? render_fwd_contrib_kernel<true> : render_fwd_contrib_kernel<false>, "render_fwd_contrib", 1,
+                                                 contrib_out(cb));
+                              const int ppl = g_ppl_fwd.load(), uf = g_u_fwd.load();
+                              if (ppl == 4) return fwd(lazy ? render_fwd_kernel<4, 1, true> : render_fwd_kernel<4, 1, false>, "render_fwd", 4);
+                              if (ppl == 2) return fwd(lazy ? render_fwd_kernel<2, 2, true> : render_fwd_kernel<2, 2, false>, "render_fwd", 2);
+                              if (uf == 4) return fwd(lazy ? render_fwd_kernel<1, 4, true> : render_fwd_kernel<1, 4, false>, "render_fwd", 1);
+                              // default <1,1>: 58 registers, 8 CTAs per SM, no spill
+                              return fwd(lazy ? render_fwd_kernel<1, 1, true> : render_fwd_kernel<1, 1, false>, "render_fwd", 1);
+                          },
+                          H, W, IL.gx);
 }
 
 int dgr_forward_render(const DgrSettings *s, const DgrGaussians *g, void *geom_v, void *binning_v, uint64_t capacity,
@@ -798,11 +875,14 @@ static int flat_segs(int32_t n_seg, const int64_t *seg_off, const int32_t *seg_s
     return 0;
 }
 
-// dgr_backward (det = NULL) and dgr_backward_det
+// dgr_backward, dgr_backward_ex (det = NULL) and dgr_backward_det, dgr_backward_det_ex (opt = NULL: no options)
 static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
                            int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                           const DgrGaussianGrads *gout, const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, float *abs_accum,
-                           void *stream) {
+                           const DgrGaussianGrads *gout, const DetArgs *det, const DgrRasterOptions *opt, void *stream) {
+    uint32_t flags = 0;
+    const DgrCameraGrads *cam = nullptr;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     if (int e = check_settings(s)) return e;
     if (int e = check_gaussians(s, g)) return e;
     if (int e = check_camera(cam, 1, g->P)) return e;
@@ -812,10 +892,10 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
     if (det)
         if (int e = check_det(*det, gout, capacity, g->P)) return e;
     cudaStream_t st = (cudaStream_t)stream;
-    ViewTable vt1;                                   // the camera kernels' view table: one view of H x W
-    if (cam) { memset(&vt1, 0, sizeof(vt1)); vt1.H[0] = s->image_height; vt1.W[0] = s->image_width; }
-    if (g->P == 0)
-        return cam ? camera_grads(s, g, cam, 1, vt1, make_float2(s->tanfovx, s->tanfovy), nullptr, radii, nullptr, nullptr, false, st) : 0;
+    ViewTable vt1;                                   // one view of H x W: the view table of the statistics and camera kernels
+    memset(&vt1, 0, sizeof(vt1)); vt1.H[0] = s->image_height; vt1.W[0] = s->image_width;
+    const float2 tan0 = make_float2(s->tanfovx, s->tanfovy);
+    if (g->P == 0) return cam ? camera_grads(s, g, cam, 1, vt1, tan0, nullptr, radii, nullptr, nullptr, false, st) : 0;
     if (!radii) return fail(-1, "radii is NULL");
     if (int e = check_push(gout->push, g->P)) return e;
     char *geom = (char *)geom_v;
@@ -823,91 +903,29 @@ static int backward_single(const DgrSettings *s, const DgrGaussians *g, void *ge
     const int H = s->image_height, W = s->image_width;
     GeomLayout GL(g->P, H, W);
     ImageLayout IL(H, W);
-    BinningLayout BL(capacity);
     if (int e = check_forward_flags(image, IL, flags, s->debug, st)) return e;
-    const int tiles = IL.gx * IL.gy;
-    float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
-    // one memset: the work counter of the persistent backward render kernel + the per-Gaussian moment accumulators
-    DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * kGradRecFloats * 4, st));
-    if (det && binning && capacity > 0) {
-        DevInfo *dv = dev_info();
-        if (!dv) return -1;
-        if (int e = det_render(dv, *det, g->P, H, W, IL.gx, nullptr, tiles, image, IL, geom, GL, binning, BL, staging == DGR_STAGING_BY_ID,
-                               s->bg, gin, grad_rec, abs_accum != nullptr, s->debug, st)) return e;
-    } else if (binning && capacity > 0) {
-        DevInfo *dv = dev_info();
-        if (!dv) return -1;
-        const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
-        unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
-        const int ppl = g_ppl_bwd.load(), ub = g_u_bwd.load();
-        const CostOrder co = cost_order(image, IL, tiles, ppl == 1 ? 1 : 2);     // (the kernel checks that the forward grouped its costs for this shape)
-#define DGR_RENDER_BWD_L(PPL_, U_, L_)                                                                                        \
-    do {                                                                                                                   \
-        const size_t smem_ = sizeof(BwdSmem<PPL_>) * kRenderWarps;                                                         \
-        int grid_ = min(persistent_grid(dv, render_bwd_kernel<PPL_, U_, L_>, kRenderThreads, smem_),                       \
-                        (tiles * SubTile<PPL_>::kPerTile + kRenderWarps - 1) / kRenderWarps);                              \
-        if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);                                          \
-        DGR_KERNEL("render_bwd", st, s->debug,                                                                             \
-                   launch_k(render_bwd_kernel<PPL_, U_, L_>, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, H, W, IL.gx, \
-                            reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co, \
-                            reinterpret_cast<const uint2 *>(image + IL.off_oranges),                                       \
-                            reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec), \
-                            (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),          \
-                            s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),                                 \
-                            reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, grad_rec)); \
-    } while (0)
-#define DGR_RENDER_BWD(PPL_, U_) do { if (lazy) DGR_RENDER_BWD_L(PPL_, U_, true); else DGR_RENDER_BWD_L(PPL_, U_, false); } while (0)
-        // the record staging the forward chose (dgr_forward_render): only then does the sorted copy exist
-        const bool lazy = staging == DGR_STAGING_BY_ID;
-        if (abs_accum) {                                               // DGR_RASTER_ABS_GRAD: the default shape's ABS variant, whatever the knobs
-            const CostOrder co1 = cost_order(image, IL, tiles, 1);
-            auto launch = [&](auto kernel) -> int {
-                const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;
-                int grid_ = min(persistent_grid(dv, kernel, kRenderThreads, smem_), (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);
-                if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);
-                DGR_KERNEL("render_bwd_abs", st, s->debug,
-                           launch_k(kernel, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, H, W, IL.gx,
-                                    reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co1,
-                                    reinterpret_cast<const uint2 *>(image + IL.off_oranges),
-                                    reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec),
-                                    (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),
-                                    s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),
-                                    reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, grad_rec));
-                return 0;
-            };
-            if (int e = lazy ? launch(render_bwd_abs_kernel<true>) : launch(render_bwd_abs_kernel<false>)) return e;
-        } else
-        if (ppl == 1 && ub != 1 && !lazy && !g_rowsum.load()) {       // A/B: the default shape with the per-pixel step 2
-#define DGR_BWD_OLD_ render_bwd_kernel<1, 2, false, false>
-            const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;
-            int grid_ = min(persistent_grid(dv, DGR_BWD_OLD_, kRenderThreads, smem_), (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);
-            if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);
-            DGR_KERNEL("render_bwd", st, s->debug,
-                       launch_k(DGR_BWD_OLD_, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, H, W, IL.gx,
-                                reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co,
-                                reinterpret_cast<const uint2 *>(image + IL.off_oranges),
-                                reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec),
-                                (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),
-                                s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),
-                                reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, grad_rec));
-#undef DGR_BWD_OLD_
-        } else
-        if (ppl == 1) { if (ub == 1) DGR_RENDER_BWD(1, 1); else DGR_RENDER_BWD(1, 2); }     // default <1,2> (in-pipeline sweep, profiles/r2_sweep.txt)
-        else { if (ub == 2) DGR_RENDER_BWD(2, 2); else DGR_RENDER_BWD(2, 1); }
-#undef DGR_RENDER_BWD_L
-#undef DGR_RENDER_BWD
-    }
-    const bool aa = flags & DGR_RASTER_ANTIALIAS;
-    DGR_KERNEL("preprocess_bwd", st, s->debug, DGR_DISPATCH(launch_pre_bwd, s, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout, aa, st));
-    if (abs_accum) {
-        ViewTable vt_abs;                            // one view of H x W
-        memset(&vt_abs, 0, sizeof(vt_abs)); vt_abs.H[0] = H; vt_abs.W[0] = W;
-        if (int e = absgrad_stats(g->P, 1, vt_abs, 1u, radii, grad_rec, abs_accum, s->debug, st)) return e;
-    }
-    if (cam)
-        return camera_grads(s, g, cam, 1, vt1, make_float2(s->tanfovx, s->tanfovy), nullptr, radii,
-                            reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, aa, st);
-    return 0;
+    return backward_stages(
+        s, g, 1, vt1, tan0, nullptr, 1u, geom, GL, image, IL, binning, capacity, staging, radii, gin, det, flags, cam, abs_accum, st,
+        [&](auto bwd, bool lazy) {
+            // DGR_RASTER_ABS_GRAD: the default shape's ABS variant, whatever the knobs
+            if (abs_accum) return bwd(lazy ? render_bwd_abs_kernel<true> : render_bwd_abs_kernel<false>, "render_bwd_abs", 1);
+            const int ppl = g_ppl_bwd.load(), ub = g_u_bwd.load();
+            // A/B: the default shape with the per-pixel step 2
+            if (ppl == 1 && ub != 1 && !lazy && !g_rowsum.load()) return bwd(render_bwd_kernel<1, 2, false, false>, "render_bwd", 1);
+            if (ppl == 1) {                              // default <1,2> (in-pipeline sweep, profiles/r2_sweep.txt)
+                if (ub == 1) return bwd(lazy ? render_bwd_kernel<1, 1, true> : render_bwd_kernel<1, 1, false>, "render_bwd", 1);
+                return bwd(lazy ? render_bwd_kernel<1, 2, true> : render_bwd_kernel<1, 2, false>, "render_bwd", 1);
+            }
+            if (ub == 2) return bwd(lazy ? render_bwd_kernel<2, 2, true> : render_bwd_kernel<2, 2, false>, "render_bwd", 2);
+            return bwd(lazy ? render_bwd_kernel<2, 1, true> : render_bwd_kernel<2, 1, false>, "render_bwd", 2);
+        },
+        [&](const unsigned *touched, const float *grad_rec, bool aa) -> int {
+            DGR_KERNEL("preprocess_bwd", st, s->debug, dispatch_gaussians(s->sh_degree, g, [&](auto deg, auto sh, auto cov, auto raw) {
+                launch_pre_bwd<deg, sh, cov, raw>(s, g, radii, touched, grad_rec, gout, aa, st);
+            }));
+            return 0;
+        },
+        H, W, IL.gx);
 }
 
 int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -915,7 +933,7 @@ int dgr_backward(const DgrSettings *s, const DgrGaussians *g, void *geom_v, cons
                  const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_backward");
     (void)out_alpha;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, nullptr, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, nullptr, stream);
 }
 
 int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -923,11 +941,7 @@ int dgr_backward_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, c
                     const DgrGaussianGrads *gout, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_backward_ex");
     (void)out_alpha;
-    uint32_t flags = 0;
-    const DgrCameraGrads *cam = nullptr;
-    float *abs_accum = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, abs_accum, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, opt, stream);
 }
 
 size_t dgr_det_scratch_bytes(uint64_t instances, int64_t records) { return DetLayout(instances, records).total; }
@@ -939,7 +953,7 @@ int dgr_backward_det(const DgrSettings *s, const DgrGaussians *g, void *geom_v, 
     NvtxRange nvtx_("dgr_backward_det");
     (void)out_alpha;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, nullptr, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, nullptr, stream);
 }
 
 int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -948,12 +962,8 @@ int dgr_backward_det_ex(const DgrSettings *s, const DgrGaussians *g, void *geom_
                         const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_backward_det_ex");
     (void)out_alpha;
-    uint32_t flags = 0;
-    const DgrCameraGrads *cam = nullptr;
-    float *abs_accum = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, abs_accum, stream);
+    return backward_single(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, opt, stream);
 }
 
 }  // extern "C"
@@ -1083,22 +1093,6 @@ void launch_views_pre_bwd(const DgrViews *s, const ViewsBatch &b, const DgrGauss
              o->denom, o->max_radii2D, (unsigned long long)stats_views, o->accumulate);
 }
 
-#define DGR_VIEWS_DISPATCH(FN, ...)                                                                        \
-    do {                                                                                                   \
-        if (g->activations) switch (s->sh_degree) {                                                        \
-            case 0: FN<0, true>(__VA_ARGS__); break;                                                       \
-            case 1: FN<1, true>(__VA_ARGS__); break;                                                       \
-            case 2: FN<2, true>(__VA_ARGS__); break;                                                       \
-            default: FN<3, true>(__VA_ARGS__); break;                                                      \
-        }                                                                                                  \
-        else switch (s->sh_degree) {                                                                       \
-            case 0: FN<0, false>(__VA_ARGS__); break;                                                      \
-            case 1: FN<1, false>(__VA_ARGS__); break;                                                      \
-            case 2: FN<2, false>(__VA_ARGS__); break;                                                      \
-            default: FN<3, false>(__VA_ARGS__); break;                                                     \
-        }                                                                                                  \
-    } while (0)
-
 // The three stages of a checked batch (s, g and the sizes in b).
 int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, void *image_v, int32_t *radii, uint32_t flags,
                      void *stream) {
@@ -1113,7 +1107,9 @@ int views_preprocess(const DgrViews *s, const ViewsBatch &b, const DgrGaussians 
     const bool aa = flags & DGR_RASTER_ANTIALIAS;
     if (g->P > 0)
         DGR_KERNEL("preprocess_views_fwd", st, s->debug,
-                   DGR_VIEWS_DISPATCH(launch_views_pre_fwd, s, b, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), aa, st));
+                   dispatch_views(s->sh_degree, g->activations, [&](auto deg, auto raw) {
+                       launch_views_pre_fwd<deg, raw>(s, b, g, radii, geom, L, reinterpret_cast<unsigned *>(image + IL.off_count), aa, st);
+                   }));
     return 0;
 }
 
@@ -1131,67 +1127,15 @@ int views_render(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, 
     char *geom = (char *)geom_v, *binning = (char *)binning_v, *image = (char *)image_v;
     const GeomLayout GL = GeomLayout::batch(g->P, b.tiles, s->V);
     const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
-    BinningLayout BL(capacity);
-    const int tiles = b.tiles;
-    uint2 *ranges = reinterpret_cast<uint2 *>(image + IL.off_ranges);
-    unsigned *tile_count = reinterpret_cast<unsigned *>(image + IL.off_count);
-    const unsigned *run_matrix = reinterpret_cast<const unsigned *>(geom + GL.off_runs);
-    GeomHeader *hdr = reinterpret_cast<GeomHeader *>(geom);
-    const Rec *rec = reinterpret_cast<const Rec *>(geom + GL.off_rec);
-    unsigned long long *keys = binning ? reinterpret_cast<unsigned long long *>(binning + BL.off_keys) : nullptr;
-    unsigned *ids = binning ? reinterpret_cast<unsigned *>(binning + BL.off_ids) : nullptr;
-    Rec *recs = binning ? reinterpret_cast<Rec *>(binning + BL.off_rec) : nullptr;
-    unsigned *tile_order = reinterpret_cast<unsigned *>(image + IL.off_order);
-    unsigned *big_list = reinterpret_cast<unsigned *>(image + IL.off_biglist);
-    TileWork *work = reinterpret_cast<TileWork *>(image + IL.off_work);
-    DevInfo *dv = dev_info();
-    if (!dv) return -1;
-    if (flags & DGR_FLAG_RERUN)
-        if (int e = clear_costs_for_rerun(image, IL, tiles, st)) return e;
-    if (int e = contrib_clear(cb, records, st)) return e;
-    {
-        const int nb = (g->P > 0 && capacity > 0) ? GL.nblocks : 0;
-        DGR_KERNEL("emit_views", st, s->debug,
-                   launch_k(emit_views_kernel, dim3(nb + 1), dim3(kPreThreads), (size_t)tiles * 4, st, !(flags & DGR_FLAG_RERUN), g->P, s->V, b.vt,
-                            GL.iters, nb, rec, reinterpret_cast<const unsigned *>(geom + GL.off_touched), (const unsigned *)tile_count,
-                            (unsigned long long)capacity, run_matrix, keys, ranges, hdr, tile_order, reinterpret_cast<uint2 *>(image + IL.off_oranges),
-                            work, big_list, (volatile unsigned long long *)(ticket ? counts_host : nullptr), (unsigned long long)ticket));
-    }
-    if (int e = copy_counts(geom, counts_host, ticket, count_ready_event, st)) return e;
-    const bool lazy = stage_records_by_id(capacity, dv, counts_host);
-    if (g->P > 0 && capacity > 0)
-        if (int e = launch_tile_sorts(dv, image, IL, tiles, flags & DGR_FLAG_BIG_TILES, lazy, keys, rec, ids, recs, s->debug, st)) return e;
-    const CostOrder co = cost_order(image, IL, tiles, 1);          // the batched backward's 8x4 sub-tiles
-#define DGR_VIEWS_FWD(L_)                                                                                                   \
-    do {                                                                                                                   \
-        const int items_ = tiles * SubTile<1>::kPerTile;                                                                   \
-        int grid_ = min(persistent_grid(dv, render_views_fwd_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
-        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                                          \
-        DGR_KERNEL("render_views_fwd", st, s->debug,                                                                       \
-                   launch_k(render_views_fwd_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, b.vt,         \
-                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),          \
-                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
-                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids, s->bg, out->color, out->depth, out->alpha, \
-                            reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT))); \
-    } while (0)
-#define DGR_VIEWS_FWD_C(L_)                                                                                                 \
-    do {                                                                                                                   \
-        const int items_ = tiles * SubTile<1>::kPerTile;                                                                   \
-        int grid_ = min(persistent_grid(dv, render_views_fwd_contrib_kernel<L_>, kRenderThreads, 0), (items_ + kRenderWarps - 1) / kRenderWarps); \
-        if (g_cta_fwd.load() > 0) grid_ = min(grid_, g_cta_fwd.load() * dv->sms);                                          \
-        DGR_KERNEL("render_views_fwd_contrib", st, s->debug,                                                               \
-                   launch_k(render_views_fwd_contrib_kernel<L_>, dim3((unsigned)grid_), dim3(kRenderThreads), 0, st, true, b.vt, \
-                            (const unsigned *)tile_order, reinterpret_cast<const uint2 *>(image + IL.off_oranges),          \
-                            (const unsigned *)&work->n_nonempty, (unsigned)items_, &work->fwd_next, g_two_ended.load(), dv->sms, co, \
-                            &work->lazy, (const Rec *)recs, rec, (const unsigned *)ids, s->bg, out->color, out->depth, out->alpha, \
-                            reinterpret_cast<unsigned *>(image + IL.off_ncontrib), reinterpret_cast<float *>(image + IL.off_finalT), \
-                            contrib_out(cb)));                                                                               \
-    } while (0)
-    if (cb) { if (lazy) DGR_VIEWS_FWD_C(true); else DGR_VIEWS_FWD_C(false); }
-    else if (lazy) DGR_VIEWS_FWD(true); else DGR_VIEWS_FWD(false);
-#undef DGR_VIEWS_FWD
-#undef DGR_VIEWS_FWD_C
-    return contrib_finalize(cb, records, s->debug, st);
+    return forward_stage2(s, g->P, records, geom, GL, image, IL, binning, capacity, flags, counts_host, ticket, count_ready_event, out, cb,
+                          1, st,                 // the batched backward's 8x4 sub-tiles
+                          [&](auto emit) { return emit(emit_views_kernel, "emit_views", g->P, s->V, b.vt); },
+                          [&](auto fwd, bool lazy) {
+                              if (cb) return fwd(lazy ? render_views_fwd_contrib_kernel<true> : render_views_fwd_contrib_kernel<false>,
+                                                 "render_views_fwd_contrib", 1, contrib_out(cb));
+                              return fwd(lazy ? render_views_fwd_kernel<true> : render_views_fwd_kernel<false>, "render_views_fwd", 1);
+                          },
+                          b.vt);
 }
 
 int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity,
@@ -1207,58 +1151,22 @@ int views_backward(const DgrViews *s, const ViewsBatch &b, const DgrGaussians *g
     const char *binning = (const char *)binning_v, *image = (const char *)image_v;
     const GeomLayout GL = GeomLayout::batch(g->P, b.tiles, s->V);
     const ImageLayout IL = ImageLayout::batch((size_t)b.tiles, b.pixels);
-    BinningLayout BL(capacity);
     if (int e = check_forward_flags(image, IL, flags, s->debug, st)) return e;
-    const int tiles = b.tiles;
-    float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
-    DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)g->P * s->V * kGradRecFloats * 4, st));
-    if (det && binning && capacity > 0) {
-        DevInfo *dv = dev_info();
-        if (!dv) return -1;
-        if (int e = det_render(dv, *det, (long long)g->P * s->V, 0, 0, 0, &b.vt, tiles, image, IL, geom, GL, binning, BL,
-                               staging == DGR_STAGING_BY_ID, s->bg, gin, grad_rec, abs_accum != nullptr, s->debug, st)) return e;
-    } else if (binning && capacity > 0) {
-        DevInfo *dv = dev_info();
-        if (!dv) return -1;
-        const TileWork *work = reinterpret_cast<const TileWork *>(image + IL.off_work);
-        unsigned long long *bwd_next = reinterpret_cast<unsigned long long *>(geom + GL.off_bwdwork);
-        const CostOrder co = cost_order(image, IL, tiles, 1);
-        const bool lazy = staging == DGR_STAGING_BY_ID;
-#define DGR_VIEWS_BWD_K(K_, NAME_)                                                                                              \
-    do {                                                                                                                       \
-        const size_t smem_ = sizeof(BwdSmem<1>) * kRenderWarps;                                                                \
-        int grid_ = min(persistent_grid(dv, K_, kRenderThreads, smem_),                                                        \
-                        (tiles * SubTile<1>::kPerTile + kRenderWarps - 1) / kRenderWarps);                                     \
-        if (g_cta_bwd.load() > 0) grid_ = min(grid_, g_cta_bwd.load() * dv->sms);                                              \
-        DGR_KERNEL(NAME_, st, s->debug,                                                                                        \
-                   launch_k(K_, dim3((unsigned)grid_), dim3(kRenderThreads), smem_, st, false, b.vt,                           \
-                            reinterpret_cast<const unsigned *>(image + IL.off_order), &work->n_nonempty, bwd_next, g_two_ended.load(), dv->sms, co, \
-                            reinterpret_cast<const uint2 *>(image + IL.off_oranges),                                           \
-                            reinterpret_cast<const Rec *>(binning + BL.off_rec), reinterpret_cast<const Rec *>(geom + GL.off_rec), \
-                            (const unsigned *)&work->lazy, reinterpret_cast<const unsigned *>(binning + BL.off_ids),             \
-                            s->bg, reinterpret_cast<const float *>(image + IL.off_finalT),                                     \
-                            reinterpret_cast<const unsigned *>(image + IL.off_ncontrib), gin->dL_dcolor, gin->dL_ddepth, gin->dL_dalpha, \
-                            grad_rec));                                                                                        \
-    } while (0)
-        if (abs_accum) {                             // DGR_RASTER_ABS_GRAD: the ABS variant of the same kernel
-            if (lazy) DGR_VIEWS_BWD_K(render_views_bwd_abs_kernel<true>, "render_views_bwd_abs");
-            else DGR_VIEWS_BWD_K(render_views_bwd_abs_kernel<false>, "render_views_bwd_abs");
-        } else {
-            if (lazy) DGR_VIEWS_BWD_K(render_views_bwd_kernel<true>, "render_views_bwd");
-            else DGR_VIEWS_BWD_K(render_views_bwd_kernel<false>, "render_views_bwd");
-        }
-#undef DGR_VIEWS_BWD_K
-    }
-    const bool aa = flags & DGR_RASTER_ANTIALIAS;
-    DGR_KERNEL("preprocess_views_bwd", st, s->debug,
-               DGR_VIEWS_DISPATCH(launch_views_pre_bwd, s, b, g, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched), grad_rec, gout,
-                                  stats_views, aa, st));
-    if (abs_accum)
-        if (int e = absgrad_stats(g->P, s->V, b.vt, stats_views, radii, grad_rec, abs_accum, s->debug, st)) return e;
-    if (cam)
-        return camera_grads(s, g, cam, s->V, b.vt, make_float2(0.f, 0.f), s->tanfov, radii, reinterpret_cast<const unsigned *>(geom + GL.off_touched),
-                            grad_rec, aa, st);
-    return 0;
+    return backward_stages(
+        s, g, s->V, b.vt, make_float2(0.f, 0.f), s->tanfov, stats_views, geom, GL, image, IL, binning, capacity, staging, radii, gin, det, flags,
+        cam, abs_accum, st,
+        [&](auto bwd, bool lazy) {
+            // DGR_RASTER_ABS_GRAD: the ABS variant of the same kernel
+            if (abs_accum) return bwd(lazy ? render_views_bwd_abs_kernel<true> : render_views_bwd_abs_kernel<false>, "render_views_bwd_abs", 1);
+            return bwd(lazy ? render_views_bwd_kernel<true> : render_views_bwd_kernel<false>, "render_views_bwd", 1);
+        },
+        [&](const unsigned *touched, const float *grad_rec, bool aa) -> int {
+            DGR_KERNEL("preprocess_views_bwd", st, s->debug, dispatch_views(s->sh_degree, g->activations, [&](auto deg, auto raw) {
+                launch_views_pre_bwd<deg, raw>(s, b, g, radii, touched, grad_rec, gout, stats_views, aa, st);
+            }));
+            return 0;
+        },
+        b.vt);
 }
 }  // namespace
 
@@ -1305,9 +1213,14 @@ int dgr_views_forward_render_ex(const DgrViews *s, const DgrGaussians *g, void *
                         count_ready_event, opt, stream);
 }
 
+// dgr_views_backward* (det = NULL: not deterministic, opt = NULL: no options)
 static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                                const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
-                               const DetArgs *det, uint32_t flags, const DgrCameraGrads *cam, const float *abs_accum, void *stream) {
+                               const DetArgs *det, const DgrRasterOptions *opt, void *stream) {
+    uint32_t flags = 0;
+    const DgrCameraGrads *cam = nullptr;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     if (int e = check_views(s)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1325,18 +1238,14 @@ static int views_backward_same(const DgrViews *s, const DgrGaussians *g, void *g
 int dgr_views_backward(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                        const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout, void *stream) {
     NvtxRange nvtx_("dgr_views_backward");
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, 0u, nullptr, nullptr, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, nullptr, stream);
 }
 
 int dgr_views_backward_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                           const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
                           const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_ex");
-    uint32_t flags = 0;
-    const DgrCameraGrads *cam = nullptr;
-    float *abs_accum = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, flags, cam, abs_accum, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, nullptr, opt, stream);
 }
 
 int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
@@ -1344,19 +1253,15 @@ int dgr_views_backward_det(const DgrViews *s, const DgrGaussians *g, void *geom_
                            void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, 0u, nullptr, nullptr, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, nullptr, stream);
 }
 
 int dgr_views_backward_det_ex(const DgrViews *s, const DgrGaussians *g, void *geom_v, const void *binning_v, uint64_t capacity, int32_t staging,
                               const void *image_v, const int32_t *radii, const DgrImageGrads *gin, const DgrGaussianGrads *gout,
                               void *det_scratch, uint64_t det_scratch_bytes, uint64_t instances, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_backward_det_ex");
-    uint32_t flags = 0;
-    const DgrCameraGrads *cam = nullptr;
-    float *abs_accum = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, flags, cam, abs_accum, stream);
+    return views_backward_same(s, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, &det, opt, stream);
 }
 
 // ---- views of different sizes: image_hw = [V,2] (height, width) on the host ------------------------------------------------------
@@ -1412,10 +1317,15 @@ int dgr_views_mixed_forward_render_ex(const DgrViews *s, const int32_t *image_hw
                         count_ready_event, opt, stream);
 }
 
+// dgr_views_mixed_backward* (det = NULL: not deterministic, opt = NULL: no options)
 static int views_backward_mixed(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
                                 uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
-                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, uint32_t flags,
-                                const DgrCameraGrads *cam, float *abs_accum, void *stream) {
+                                const DgrGaussianGrads *gout, uint64_t stats_views, const DetArgs *det, const DgrRasterOptions *opt,
+                                void *stream) {
+    uint32_t flags = 0;
+    const DgrCameraGrads *cam = nullptr;
+    float *abs_accum = nullptr;
+    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     if (int e = check_views_mixed(s, image_hw)) return e;
     if (int e = check_views_gaussians(s, g)) return e;
     if (!geom_v || !image_v || !gin || !gout) return fail(-1, "NULL argument");
@@ -1437,20 +1347,16 @@ int dgr_views_mixed_backward(const DgrViews *s, const int32_t *image_hw, const D
                              uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
                              const DgrGaussianGrads *gout, uint64_t stats_views, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward");
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, 0u,
-                                nullptr, nullptr, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, nullptr,
+                                stream);
 }
 
 int dgr_views_mixed_backward_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
                                 uint64_t capacity, int32_t staging, const void *image_v, const int32_t *radii, const DgrImageGrads *gin,
                                 const DgrGaussianGrads *gout, uint64_t stats_views, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_ex");
-    uint32_t flags = 0;
-    const DgrCameraGrads *cam = nullptr;
-    float *abs_accum = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, flags,
-                                cam, abs_accum, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, nullptr, opt,
+                                stream);
 }
 
 int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1459,8 +1365,8 @@ int dgr_views_mixed_backward_det(const DgrViews *s, const int32_t *image_hw, con
                                  uint64_t instances, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_det");
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, 0u, nullptr,
-                                nullptr, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, nullptr,
+                                stream);
 }
 
 int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, const DgrGaussians *g, void *geom_v, const void *binning_v,
@@ -1468,13 +1374,9 @@ int dgr_views_mixed_backward_det_ex(const DgrViews *s, const int32_t *image_hw, 
                                     const DgrGaussianGrads *gout, uint64_t stats_views, void *det_scratch, uint64_t det_scratch_bytes,
                                     uint64_t instances, const DgrRasterOptions *opt, void *stream) {
     NvtxRange nvtx_("dgr_views_mixed_backward_det_ex");
-    uint32_t flags = 0;
-    const DgrCameraGrads *cam = nullptr;
-    float *abs_accum = nullptr;
-    if (int e = raster_flags_bwd(opt, &flags, &cam, &abs_accum)) return e;
     const DetArgs det{det_scratch, det_scratch_bytes, instances};
-    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, flags,
-                                cam, abs_accum, stream);
+    return views_backward_mixed(s, image_hw, g, geom_v, binning_v, capacity, staging, image_v, radii, gin, gout, stats_views, &det, opt,
+                                stream);
 }
 
 }  // extern "C"
