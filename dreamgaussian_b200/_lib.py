@@ -310,6 +310,50 @@ def check_mcmc(code):
         raise RuntimeError("libdgr_mcmc: %s (code %d)" % (load_mcmc().dgr_mcmc_last_error().decode(), code))
 
 
+MESH_EXPORTS = ("dgr_mesh_last_error", "dgr_mesh_scratch_bytes", "dgr_mesh_marching_cubes_count", "dgr_mesh_marching_cubes_emit",
+                "dgr_mesh_components_scratch_bytes", "dgr_mesh_remove_components_count", "dgr_mesh_remove_components_emit")
+_mesh = None
+
+
+def load_mesh():
+    """Load libdgr_mesh.so (include/dgr_mesh.h: marching cubes and small-component removal), building it first when its sources
+    are newer.  Raises on failure: there is no other implementation of these entry points."""
+    global _mesh
+    if _mesh is not None:
+        return _mesh
+    path = _build.MESH_LIB_PATH
+    if _build.mesh_is_stale():
+        try:
+            _build.build_mesh()
+        except Exception as e:  # noqa: BLE001
+            if not os.path.exists(path):
+                raise RuntimeError("libdgr_mesh.so is not built and could not be compiled here (%s). "
+                                   "Run `python -m dreamgaussian_b200.build` on a machine with nvcc." % e)
+    lib = ctypes.CDLL(path)
+    vp, i32, i64, sz = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_size_t
+    i64p = ctypes.POINTER(ctypes.c_int64)
+    lib.dgr_mesh_last_error.restype = ctypes.c_char_p
+    lib.dgr_mesh_scratch_bytes.restype = sz
+    lib.dgr_mesh_scratch_bytes.argtypes = [i32, i32, i32]
+    lib.dgr_mesh_marching_cubes_count.restype = ctypes.c_int
+    lib.dgr_mesh_marching_cubes_count.argtypes = [vp, i32, i32, i32, ctypes.c_float, vp, sz, i64p, vp]
+    lib.dgr_mesh_marching_cubes_emit.restype = ctypes.c_int
+    lib.dgr_mesh_marching_cubes_emit.argtypes = [vp, i32, i32, i32, ctypes.c_float, vp, sz, i64, i64, vp, vp, vp]
+    lib.dgr_mesh_components_scratch_bytes.restype = sz
+    lib.dgr_mesh_components_scratch_bytes.argtypes = [i32, i32]
+    lib.dgr_mesh_remove_components_count.restype = ctypes.c_int
+    lib.dgr_mesh_remove_components_count.argtypes = [vp, i32, vp, i32, i32, ctypes.c_double, vp, sz, i64p, vp]
+    lib.dgr_mesh_remove_components_emit.restype = ctypes.c_int
+    lib.dgr_mesh_remove_components_emit.argtypes = [vp, i32, vp, i32, vp, sz, i64, i64, vp, vp, vp]
+    _mesh = lib
+    return lib
+
+
+def check_mesh(code):
+    if code != 0:
+        raise RuntimeError("libdgr_mesh: %s (code %d)" % (load_mesh().dgr_mesh_last_error().decode(), code))
+
+
 def profile_collect(max_records=4096):
     """-> list of (kernel name, milliseconds) recorded since dgr_profile_enable(1)."""
     lib = load()

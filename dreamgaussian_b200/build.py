@@ -138,6 +138,52 @@ def build_mcmc(force=False):
     return MCMC_LIB_PATH
 
 
+# ---- the mesh export (csrc/mesh/, include/dgr_mesh.h): marching cubes and small-component removal, a library of its own like the
+# MCMC one
+MESH_DIR = os.path.join(CSRC, "mesh")
+MESH_LIB_PATH = os.path.join(LIB_DIR, "libdgr_mesh.so")
+MESH_HASH_PATH = os.path.join(LIB_DIR, "libdgr_mesh.srchash")
+
+
+def mesh_sources():
+    return sorted(os.path.join(MESH_DIR, f) for f in os.listdir(MESH_DIR) if f.endswith((".cu", ".cuh", ".h"))) + [
+        os.path.join(HERE, "..", "include", "dgr_mesh.h")]
+
+
+def _mesh_hash():
+    import hashlib
+    h = hashlib.sha256(" ".join(NVCC_FLAGS).encode())
+    for s in mesh_sources():
+        with open(s, "rb") as f:
+            h.update(os.path.basename(s).encode() + b"\0" + f.read())
+    return h.hexdigest()
+
+
+def mesh_is_stale():
+    if not os.path.exists(MESH_LIB_PATH) or not os.path.exists(MESH_HASH_PATH):
+        return True
+    with open(MESH_HASH_PATH) as f:
+        return f.read().strip() != _mesh_hash()
+
+
+def build_mesh(force=False):
+    """Compile dreamgaussian_b200/csrc/mesh/dgr_mesh_api.cu -> dreamgaussian_b200/lib/libdgr_mesh.so (sm_90a). Returns the path."""
+    if not force and not mesh_is_stale():
+        return MESH_LIB_PATH
+    os.makedirs(LIB_DIR, exist_ok=True)
+    cmd = [_nvcc()] + NVCC_FLAGS + ["-o", MESH_LIB_PATH, os.path.join(MESH_DIR, "dgr_mesh_api.cu")]
+    if os.path.exists("/usr/bin/g++"):
+        cmd += ["-ccbin", "/usr/bin/g++"]
+    proc = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    with open(os.path.join(LIB_DIR, "build_mesh.log"), "w") as f:
+        f.write(" ".join(cmd) + "\n" + proc.stdout)
+    if proc.returncode != 0:
+        raise RuntimeError("nvcc failed on the mesh library:\n" + proc.stdout[-8000:])
+    with open(MESH_HASH_PATH, "w") as f:
+        f.write(_mesh_hash())
+    return MESH_LIB_PATH
+
+
 # ---- the compiled PyTorch host layer over the C ABI (csrc/dgr_torch.cpp): g++ only, links libdgr_b200.so
 HOST_PATH = os.path.join(LIB_DIR, "dgr_torch_host.so")
 HOST_HASH = os.path.join(LIB_DIR, "dgr_torch_host.srchash")
@@ -184,3 +230,4 @@ if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose=True))
     print(build_host(force="--force" in sys.argv))
     print(build_mcmc(force="--force" in sys.argv))
+    print(build_mesh(force="--force" in sys.argv))

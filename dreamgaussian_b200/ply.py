@@ -48,6 +48,26 @@ def save_model_ply(path, gaussians):
     save_ply(path, gaussians._xyz, gaussians._features_dc, gaussians._features_rest, gaussians._opacity, gaussians._scaling, gaussians._rotation)
 
 
+def save_mesh_ply(path, v, f):
+    """A triangle mesh as binary little-endian PLY: `element vertex` with float x y z, `element face` with
+    `property list uchar int vertex_indices` (the layout trimesh's exporter writes for the reference's Mesh.write_ply, mesh.py:434-440;
+    recalled, PARITY UNPINNED as for the Gaussian PLY).  v [Nv,3], f [Nf,3] tensors or arrays."""
+    d = os.path.dirname(path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    v = np.ascontiguousarray(_np(v), dtype="<f4").reshape(-1, 3)
+    f = np.ascontiguousarray(_np(f), dtype="<i4").reshape(-1, 3)
+    rec = np.empty(f.shape[0], dtype=np.dtype([("n", "u1"), ("i", "<i4", (3,))]))
+    rec["n"] = 3
+    rec["i"] = f
+    header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+              "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % (v.shape[0], f.shape[0]))
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(rec.tobytes())
+
+
 def read_vertex_element(path):
     """Minimal PLY reader: the first element's scalar properties as a dict name -> float64/native array (ascii,
     binary_little_endian and binary_big_endian; list properties are not part of this format)."""

@@ -718,3 +718,13 @@ class Stage1Trainer:
             rasterize_views_raw(self.export_settings(resolution), g._xyz, None, g._features_dc, g._features_rest, g._opacity, g._scaling,
                                 g._rotation, antialiasing=self.cfg.antialiasing, contributions=stats)
         return g.prune_by_contribution(stats, min_weight_max)
+
+    def save_mesh(self, path, density_thresh=1.0, resolution=128):
+        """save_model(mode='geo') (main.py:405-410) without the texture half: extract_fields, marching cubes, the world transform and
+        the small-component removal on the device (meshing.extract_mesh_of_model), written as a binary PLY.  Returns (v, f).
+        train() does not call it; prune_unseen stays a separate call."""
+        from . import meshing
+        from .ply import save_mesh_ply
+        v, f = meshing.extract_mesh_of_model(self.gaussians, density_thresh, resolution)
+        save_mesh_ply(path, v, f)
+        return v, f
