@@ -671,6 +671,8 @@ int backward_stages(const S *s, const DgrGaussians *g, int V, const ViewTable &v
     const long long records = (long long)g->P * V;
     const int tiles = GL.tiles;
     float *grad_rec = reinterpret_cast<float *>(geom + GL.off_gradrec);
+    // the backward render adds each moment row with 16-byte vector reductions
+    if (((uintptr_t)grad_rec & 15u) != 0) return fail(-1, "geometry scratch must be 16-byte aligned");
     // one memset: the work counter of the persistent backward render kernel + the per-Gaussian moment accumulators
     DGR_CUDA(cudaMemsetAsync(geom + GL.off_bwdwork, 0, (GL.off_gradrec - GL.off_bwdwork) + (size_t)records * kGradRecFloats * 4, st));
     if (binning && capacity > 0) {

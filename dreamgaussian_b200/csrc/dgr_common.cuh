@@ -33,6 +33,7 @@ static_assert(sizeof(Rec) == 48, "Rec must be 48 bytes");
 //   6..8 sum w * dL/dC[rgb] 9 sum w * dL/dD        10, 11 unused
 // with u = o * G * dL/dalpha, w = alpha * T, d = mean_px - pixel.
 constexpr int kGradRecFloats = 12;
+static_assert(kGradRecFloats * 4 % 16 == 0, "moment rows stay 16-byte aligned for the vector reductions of the backward render");
 
 struct GeomHeader {
     unsigned long long n_inst;     // total tile instances of this frame (written by the tile scan)
@@ -210,6 +211,14 @@ __device__ __forceinline__ float rcp_approx(float x) {
 __device__ __forceinline__ int bfind_u32(unsigned x) { int r; asm("bfind.u32 %0, %1;" : "=r"(r) : "r"(x)); return r; }
 __device__ __forceinline__ void red_add_f32(float *addr, float v) {
     asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
+}
+// sm_90 vector reductions: one L2 operation adds 2 / 4 consecutive floats (SASS: REDG.E.ADD.F32x2 / F32x4).  Each float
+// receives exactly the addition the scalar form would make; addr must be 8 / 16-byte aligned.
+__device__ __forceinline__ void red_add_v2_f32(float *addr, float a, float b) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void red_add_v4_f32(float *addr, float a, float b, float c, float d) {
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 __device__ __forceinline__ float4 ldg_f4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
 // L2 residency control for the record gather of the per-tile sort: the per-Gaussian record array (48 B x P) is re-read N/P

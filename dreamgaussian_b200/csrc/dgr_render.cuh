@@ -701,12 +701,22 @@ render_bwd_body(int H, int W, int gx, const unsigned *__restrict__ tile_order, c
                 v8 += __shfl_xor_sync(0xffffffffu, v8, o); v9 += __shfl_xor_sync(0xffffffffu, v9, o);
                 if constexpr (ABS) { v10 += __shfl_xor_sync(0xffffffffu, v10, o); v11 += __shfl_xor_sync(0xffffffffu, v11, o); }
             }
+            // vector reductions (the row is 16-byte aligned, GeomLayout): L2 absorbs about as many reductions per second whatever
+            // their width, so 4 per record take 2.5x less time than 10 scalar ones (tools/red_probe.py).  The single-view by-id
+            // variant keeps the scalar form: under the 80-register cap the vector operands' register pairs and quads cost it 8 more
+            // bytes of stack (16 -> 24).
             if (lane < nslots) {
                 float *dst = grad_rec + (size_t)cap_id * kGradRecFloats;
-                red_add_f32(dst, v0); red_add_f32(dst + 1, v1); red_add_f32(dst + 2, v2); red_add_f32(dst + 3, v3);
-                red_add_f32(dst + 4, v4); red_add_f32(dst + 5, v5); red_add_f32(dst + 6, v6); red_add_f32(dst + 7, v7);
-                red_add_f32(dst + 8, v8); red_add_f32(dst + 9, v9);
-                if constexpr (ABS) { red_add_f32(dst + 10, v10); red_add_f32(dst + 11, v11); }
+                if constexpr (LAZY && !VIEWS && !ABS) {
+                    red_add_f32(dst, v0); red_add_f32(dst + 1, v1); red_add_f32(dst + 2, v2); red_add_f32(dst + 3, v3);
+                    red_add_f32(dst + 4, v4); red_add_f32(dst + 5, v5); red_add_f32(dst + 6, v6); red_add_f32(dst + 7, v7);
+                    red_add_f32(dst + 8, v8); red_add_f32(dst + 9, v9);
+                } else {
+                    red_add_v4_f32(dst, v0, v1, v2, v3);
+                    if constexpr (ABS) { red_add_v4_f32(dst + 4, v4, v5, v6, v7); red_add_v2_f32(dst + 10, v10, v11); }
+                    else { red_add_v2_f32(dst + 4, v4, v5); red_add_v2_f32(dst + 6, v6, v7); }
+                    red_add_v2_f32(dst + 8, v8, v9);
+                }
             }
             nslots = 0;
             __syncwarp();
